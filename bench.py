@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- SD1.5 PCM-LoRA distillation steps/sec on B200 (BASELINE.json metric).
+"""bench.py -- SD1.5 PCM-LoRA distillation steps/sec on H100 (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's B200 path
+    python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR   # + the last timed step's results as .npy
     python bench.py --impl reference --gpus N --steps K ...  # the reference loop restated on CPU
 
 Workload (BASELINE configs[1]): SD1.5 UNet (859.5 M params, random init), LoRA r=64 on the 278
@@ -9,7 +10,7 @@ target modules, 4-phase PCM, per-GPU batch 8, 512x512 images = 64x64x4 latents, 
 CFG solver on (2 teacher passes), Huber loss, clip 1.0, AdamW.  One "step" = the full iteration
 of train_pcm_lora_sd15.py:1139-1301 on one per-GPU batch.  `value` = per-GPU-batch steps per
 second summed over all ranks (data parallel, weak scaling: global batch = 8 x N).
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  Writes nothing into the repository tree.
 """
 import argparse
 import json
@@ -34,8 +35,9 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1370.0), d.get("bf16_tflops", 1602.4), d.get("hbm_gbs", 6589.3), "measured"
-    return 1400.0, 1590.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    # NVIDIA H100 SXM data sheet (700 W): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s -- not reached in practice
+    return 989.0, 989.0, 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -225,6 +227,26 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
+DUMP_SAMPLE = 1 << 22   # elements kept of each large output (16 MB in float32)
+
+
+def dump_outputs(step, out_dir):
+    """What the timed path hands back after its last step: the loss, the updated LoRA factors (flat fp32
+    master copy) and AdamW's moments.  Arrays larger than DUMP_SAMPLE are reduced to a fixed, seeded
+    sample of positions (the same positions for the same network), float32 throughout, < 64 MB in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": step.loss, "lora_master": step.unet.lora_master,
+              "adam_exp_avg": step.exp_avg, "adam_exp_avg_sq": step.exp_avg_sq}
+    for name, t in arrays.items():
+        t = t.detach().reshape(-1).float()
+        if t.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(1234)
+            idx = torch.randperm(t.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+            t = t[idx.to(t.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy().astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -239,7 +261,10 @@ def main():
     ap.add_argument("--multiphase", type=int, default=4)
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--profile-only", action="store_true", help="one eager step, then exit (for ncu)")
+    ap.add_argument("--profile-only", action="store_true", help="one eager step, then exit (for a profiler)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (loss, updated LoRA "
+                         "factors, AdamW moments; fixed seeded samples of the large arrays) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -305,6 +330,8 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(step, args.dump_outputs)
     if world > 1:
         t = torch.tensor([ms], device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -375,13 +402,10 @@ def main():
         tot_ms = sum(a.elapsed_time(b) for a, b, _ in recs)
         tot_fl = sum(f for _, _, f in recs)
         ach = tot_fl / (tot_ms * 1e-3) / 1e12 if tot_ms > 0 else 0.0
-        traffic = None
-        tj = os.path.join(ROOT, "profiles", "r2_gemm_traffic.json")
-        if os.path.exists(tj):   # dram__bytes_read.sum + dram__bytes_write.sum per launch, from the committed
-            traffic = json.load(open(tj)).get("dram_bytes_per_launch_mean")   # `ncu --set full` capture
-        roof = {"bound": "tensor", "kernel": "pcm_gemm_kernel (tcgen05 implicit GEMM, all conv/linear/LoRA/dgrad launches)",
+        traffic = None   # DRAM bytes per launch: not measured on this GPU
+        roof = {"bound": "tensor", "kernel": "pcm_gemm_kernel (wgmma implicit GEMM, all conv/linear/LoRA/dgrad launches)",
                 "achieved": ach, "peak": sus, "unit": "TFLOP/s", "frac": ach / sus, "traffic": traffic,
-                "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({src})", "timing": mode,
+                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if src == "measured" else src, "timing": mode,
                 "launches": len(recs), "gemm_ms_per_step": tot_ms, "gemm_flop_per_step": tot_fl,
                 "whole_step_achieved": FLOP_PER_SAMPLE_64 * B * (hw / 64.0) ** 2 / (ms_per_step * 1e-3) / 1e12,
                 "whole_step_frac": FLOP_PER_SAMPLE_64 * B * (hw / 64.0) ** 2 / (ms_per_step * 1e-3) / 1e12 / sus}
@@ -405,7 +429,7 @@ def main():
                                    f"({hw}x{hw}x4 latents), LoRA r=64, CFG solver on, Huber, AdamW",
                        "per_gpu_batch": B, "global_batch": B * world, "parallelism": f"dp{world}",
                        "cuda_graph": use_graph,
-                       "l2": "working set (1.7 GB weights + >10 GB activations per step) >> 126 MB L2; no flush needed",
+                       "l2": "working set (1.7 GB weights + >10 GB activations per step) >> 50 MB L2; no flush needed",
                        "value_definition": "per-GPU-batch steps/s summed over ranks"},
             "clocks": clocks, "loss": loss_last,
             "e2e": {"value": e2e_value, "unit": "steps/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4},

@@ -1,4 +1,4 @@
-/* pcm_b200 -- C ABI of the B200-native PCM-LoRA distillation hot path.
+/* pcm_b200 -- C ABI of the H100 (sm_90a) PCM-LoRA distillation hot path.
  *
  * The reference (G-U-N/Phased-Consistency-Model) has no FFI/plugin layer: its hot path is Python
  * calling diffusers/peft/torch modules.  This header is the boundary a maintainer binds instead
@@ -111,7 +111,7 @@ const char* pcm_last_error(void);
 int pcm_version(void);
 int pcm_num_sms(void);
 
-/* tcgen05 implicit GEMM / conv and LoRA wgrad */
+/* wgmma implicit GEMM / conv and LoRA wgrad */
 int pcm_gemm(const pcm_gemm_desc* d, void* stream);
 int pcm_wgrad(const pcm_wgrad_desc* d, void* stream);
 

@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure only -- never imported by the product path).
 
 CPU restatement of the PCM distillation math of the reference,
-/root/reference/code/text_to_image_sd15/train_pcm_lora_sd15.py (T15) and
+code/text_to_image_sd15/train_pcm_lora_sd15.py (T15) and
 scheduling_ddpm_modified.py (S15).  Every function cites the lines it follows.  The restatement
 is PINNED against the reference's own functions executed verbatim (AST-extracted from the
 read-only tree by tests/golden/make_golden.py -> tests/golden/pcm_math.pt; checked by

@@ -2,11 +2,11 @@
 
 Plain-PyTorch CPU restatement of the third-party modules the reference's hot path calls:
   * diffusers==0.26.3 ``UNet2DConditionModel`` in the runwayml/stable-diffusion-v1-5 configuration
-    (call sites: /root/reference/code/text_to_image_sd15/train_pcm_lora_sd15.py:1192-1198 student,
+    (call sites: code/text_to_image_sd15/train_pcm_lora_sd15.py:1192-1198 student,
     :1219-1223 / :1238-1244 teacher, :1263-1268 target; construction :840, :849), and
   * peft==0.9.0 LoRA wrappers (train_pcm_lora_sd15.py:866-885: r=lora_rank, lora_alpha=8 default,
     14 target-module suffixes, A kaiming-uniform / B zeros).
-Neither package is vendored under /root/reference nor installed here (pinned in
+Neither package is vendored in the reference repository nor installed in this environment (pinned in
 code/text_to_image_sd15/environment.yaml:40,87), so the published semantics are restated from
 SURVEY.md Appendix A (A2: UNet, A3: LoRA).  PARITY UNPINNED for the UNet itself: the reference
 ships no golden vectors or tests for it; the PCM math around it is pinned separately
@@ -16,7 +16,7 @@ Parameters live in a flat dict keyed by diffusers state-dict names; LoRA tensors
 ``<module path>.lora_A.weight`` / ``.lora_B.weight`` (peft's names minus the ``base_model.model.``
 prefix and ``.default`` infix).
 
-``emulate_bf16=True`` rounds weights and every tensor the B200 path materialises in HBM to bf16
+``emulate_bf16=True`` rounds weights and every tensor the CUDA path materialises in HBM to bf16
 (straight-through in autograd); this mirrors the reference running under bf16 autocast.
 """
 import math

@@ -1,7 +1,7 @@
 // Flash-style self / cross attention, forward and backward, for the SD1.5 UNet head sizes
 // (8 heads, d = 40 / 80 / 160; kv = tokens or 77 text tokens).  No S x S matrix is materialised.
-// Round-1 implementation on the warp-level mma.sync.m16n8k16 bf16 path with cp.async
-// double-buffered K/V tiles (the tcgen05 version of this kernel is the next step; see DESIGN.md).
+// Warp-level mma.sync.m16n8k16 bf16 tensor-core path with cp.async double-buffered K/V tiles, for the
+// head sizes the wgmma / TMA kernels (attn_wg.cu) do not cover: forward d = 160, backward d > 64.
 //
 // Replaces xformers / torch SDPA attention inside diffusers' Attention processor
 // (enabled at train_pcm_lora_sd15.py:947-961; called from the UNet forwards at :1192-1198,
@@ -540,13 +540,12 @@ static int launch_bwd(const AttnParams& p, cudaStream_t stream) {
 }  // namespace pcm
 
 namespace pcm {
-int attn_fwd_tc(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H,
-                int Sq, int Skv, int D, long long ldq, long long ldk, long long ldv, long long ldo,
-                float scale, cudaStream_t stream);
-int attn_bwd_tc(const void* q, const void* k, const void* v, const void* dout, const float* lse,
+int attn_fwd_wg(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H, int Sq,
+                int Skv, int D, long long ldq, long long ldk, long long ldv, long long ldo, float scale,
+                cudaStream_t stream);  // attn_wg.cu
+int attn_bwd_wg(const void* q, const void* k, const void* v, const void* dout, const float* lse,
                 const float* delta, void* dq, void* dk, void* dv, int B, int H, int Sq, int Skv, int D,
-                long long ldq, long long ldk, long long ldv, long long ldo, float scale,
-                cudaStream_t stream);
+                long long ldq, long long ldk, long long ldv, long long ldo, float scale, cudaStream_t stream);
 }
 using namespace pcm;
 
@@ -580,12 +579,9 @@ extern "C" int pcm_attn_fwd(const void* q, const void* k, const void* v, void* o
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
   p.scale = scale;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  static const bool legacy = getenv("PCM_ATTN_LEGACY") != nullptr;
-  if (!legacy) {
-    // tcgen05 path (d <= 80); returns 1 when the shape is not covered
-    const int rc = attn_fwd_tc(q, k, v, out, lse, B, H, Sq, Skv, D, ldq, ldk, ldv, ldo, scale, st);
-    if (rc <= 0) return rc;
-  }
+  // wgmma / TMA kernel (d <= 128); returns 1 when the shape or layout is not covered
+  const int rc = attn_fwd_wg(q, k, v, out, lse, B, H, Sq, Skv, D, ldq, ldk, ldv, ldo, scale, st);
+  if (rc <= 0) return rc;
   DISPATCH_DP(D, launch_fwd);
 }
 
@@ -608,12 +604,11 @@ extern "C" int pcm_attn_bwd(const void* q, const void* k, const void* v, const v
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
   p.scale = scale;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  static const bool legacy = getenv("PCM_ATTN_LEGACY") != nullptr || getenv("PCM_ATTN_BWD_LEGACY") != nullptr;
-  if (!legacy && D <= 64 && D % 8 == 0) {
+  if (D <= 64 && D % 8 == 0) {
+    // wgmma / TMA kernels (d <= 64) after delta = rowsum(dO o O); return 1 when the layout is not covered
     const long long total = static_cast<long long>(B) * Sq * H;
     CUDA_TRY(launch_pdl(attn_delta_kernel, dim3(static_cast<unsigned>((total + 127) / 128)), dim3(128), 0, st, p));
-    const int rc = attn_bwd_tc(q, k, v, dout, lse, delta, dq, dk, dv, B, H, Sq, Skv, D, ldq, ldk, ldv, ldo,
-                               scale, st);
+    const int rc = attn_bwd_wg(q, k, v, dout, lse, delta, dq, dk, dv, B, H, Sq, Skv, D, ldq, ldk, ldv, ldo, scale, st);
     if (rc <= 0) return rc;
   }
   DISPATCH_DP(D, launch_bwd);

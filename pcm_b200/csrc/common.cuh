@@ -1,5 +1,5 @@
-// Common device helpers for the pcm_b200 sm_100a kernels: mbarrier, TMA, tcgen05/TMEM PTX wrappers.
-// Everything here is raw inline PTX for sm_100a; no CUTLASS dependency.
+// Common device helpers for the pcm_b200 sm_90a kernels: mbarrier, TMA, wgmma PTX wrappers.
+// Everything here is raw inline PTX for sm_90a; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -41,7 +41,7 @@ __device__ __forceinline__ bool elect_one() {
 
 // ---------------- programmatic dependent launch (PDL) ----------------
 // Every kernel of this library is launched with programmatic stream serialization: its prologue
-// (barrier init, TMEM allocation, descriptor prefetch) may overlap the tail of the previous kernel.
+// (barrier init, descriptor prefetch) may overlap the tail of the previous kernel.
 // griddep_sync() must be executed before the first global-memory access.
 __device__ __forceinline__ void griddep_sync() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -144,97 +144,48 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-// ---------------- tcgen05 / TMEM ----------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
+// ---------------- wgmma (warpgroup MMA, sm_90a) ----------------
+// Order this warpgroup's register / shared-memory accesses before the wgmma that follow.
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
+// Wait until at most N committed wgmma groups of this warpgroup are still in flight.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; kind::f16 covers fp16/bf16 inputs with fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <- lane i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// Keep the accumulator registers live across the asynchronous wgmma (no reordering by the compiler).
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Shared-memory matrix descriptor (sm_100 UMMA), SWIZZLE_128B, 16-bit elements.
+// Per-thread register budget of the calling warpgroup (producer warpgroups give registers up so
+// that the consumer warpgroups can hold a 64 x 256 fp32 accumulator without spilling).
+template <int R>
+__device__ __forceinline__ void regs_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void regs_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+
+// Shared-memory matrix descriptor (sm_90 wgmma), SWIZZLE_128B, 16-bit elements.
 //  K-major operand : rows of 64 elements (128 B), 8-row core groups 1024 B apart (SBO), LBO unused.
 //  MN-major operand: 128 B rows hold 64 consecutive MN elements at fixed k; 8 k-rows = 1024 B (SBO);
 //                    the next 64-wide MN group starts LBO bytes later.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                    uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
+                                                     uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;  // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;  // SWIZZLE_128B
-  return d;
-}
-
-// Instruction descriptor for kind::f16, BF16 x BF16 -> FP32.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_bf16(int m, int n, int a_mn_major,
-                                                             int b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;   // D format: F32
-  d |= 1u << 7;   // A format: BF16
-  d |= 1u << 10;  // B format: BF16
-  d |= static_cast<uint32_t>(a_mn_major & 1) << 15;
-  d |= static_cast<uint32_t>(b_mn_major & 1) << 16;
-  d |= static_cast<uint32_t>(n >> 3) << 17;
-  d |= static_cast<uint32_t>(m >> 4) << 24;
+  d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
   return d;
 }
 

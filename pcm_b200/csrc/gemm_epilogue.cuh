@@ -1,28 +1,27 @@
-// Epilogue of one 128 x block_n accumulator tile, shared by the 1-CTA and 2-CTA GEMM kernels.
+// Epilogue of one 64 x BN accumulator half-tile held in the registers of one consumer warpgroup.
 // Two phases per 32-column chunk so that global traffic is coalesced:
-//   1. each thread owns one accumulator row (TMEM lane): TMEM -> registers -> fp32 staging tile in
-//      shared memory (16-byte chunks XOR-swizzled by row to stay conflict free);
-//   2. the 128 threads of an epilogue group re-map to (row, 8-column group): 4 neighbouring lanes
-//      cover 64 contiguous output bytes of one row, add bias / row vector / residual, apply the
-//      activation, store 16 bytes.
-// Two groups of 4 warps take the even / odd chunks of the tile (grp = 0 / 1).
+//   1. every thread writes its wgmma fragments of the chunk (2 rows x 8 columns) into an fp32 staging
+//      tile in shared memory (16-byte chunks XOR-swizzled by row to stay conflict free);
+//   2. the 128 threads of the warpgroup re-map to (row, 8-column group): 4 neighbouring lanes cover
+//      64 contiguous output bytes of one row, add bias / row vector / residual, apply the activation,
+//      store 16 bytes.
 //
-// Small-K GEMMs are bound by this code, and it is instruction-fetch sensitive (ncu: 35 % of the
-// samples were `stall_no_inst` with a 14 k-instruction kernel), so the common case - bf16 output,
-// full 32-column chunk, no activation, no split-K - is a compact straight-line path and everything else (ragged N,
-// fp32 output, split-K partial sums) lives in one out-of-line routine with rolled loops.
+// The common case - bf16 output, full 32-column chunk, no activation, no split-K - is a compact
+// straight-line path and everything else (ragged N, fp32 output, split-K partial sums) lives in one
+// out-of-line routine with rolled loops.
 #pragma once
 #include "gemm_params.h"
 
 namespace pcm {
 
-// Generic phase 2 of one chunk for the calling thread's 4 rows: ragged N, fp32 output, split-K.
-static __device__ __noinline__ void gemm_epilogue_rows_generic(const GemmParams& p, const float* sb, int tm,
-                                                        int n, int r0, int cg, float* ws) {
+// Generic phase 2 of one chunk for the calling thread's 2 rows: ragged N, fp32 output, split-K.
+// m0: first output row of this warpgroup's half-tile.
+static __device__ __noinline__ void gemm_epilogue_rows_generic(const GemmParams& p, const float* sb, int m0,
+                                                               int n, int r0, int cg, float* ws) {
 #pragma unroll 1
-  for (int i = 0; i < 4; ++i) {
+  for (int i = 0; i < 2; ++i) {
     const int rr = r0 + 32 * i;
-    const int m = tm * 128 + rr;
+    const int m = m0 + rr;
     if (m >= p.M) continue;
     const float* srow = sb + rr * 32;
     if (ws) {  // split-K partial sums: plain stores into this split's slice of the workspace (the
@@ -71,21 +70,24 @@ __device__ __forceinline__ void add_bf16x8(float (&f)[8], const uint4& u) {
   t = unpack_bf16x2(u.w); f[6] += t.x; f[7] += t.y;
 }
 
-template <class Release>
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, int tm, int n0, uint32_t taddr,
-                                                   float* sb, int lane, int row, int grp, int cg,
-                                                   int r0, uint64_t* tfull, uint32_t tfull_phase,
-                                                   Release release, float* ws = nullptr) {
+// acc: the m64 x BN wgmma accumulator of this warpgroup (rows m0 .. m0 + 63, columns n0 ..);
+// sb: the warpgroup's 64 x 32 fp32 staging tile; et: thread index inside the warpgroup;
+// bar: named barrier id of the warpgroup.
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, int m0, int n0, const float (&acc)[BN / 2],
+                                                   float* sb, int et, int bar, float* ws) {
   const bool has_bias = p.bias != nullptr, has_rv = p.rowvec != nullptr;
   // split-K, fp32 output and the SiLU epilogue (time-embedding MLP, M = batch) take the generic path
   const bool fast_ok = p.ws == nullptr && !p.out_fp32 && p.act == 0;
   const bool has_res = p.residual != nullptr && fast_ok;
-  long long off[4];
-  const bf16* rvp[4];
-  bool valid[4];
+  const int cg = et & 3;   // phase 2: 8-column group inside the 32-column chunk
+  const int r0 = et >> 2;  // phase 2: rows r0 and r0 + 32
+  long long off[2];
+  const bf16* rvp[2];
+  bool valid[2];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int m = tm * 128 + r0 + 32 * i;
+  for (int i = 0; i < 2; ++i) {
+    const int m = m0 + r0 + 32 * i;
     valid[i] = m < p.M;
     off[i] = 0;
     rvp[i] = nullptr;
@@ -98,21 +100,25 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, int tm, 
       if (has_rv) rvp[i] = p.rowvec + b * p.rowvec_ld;
     }
   }
-  const int nchunks = p.block_n >> 5;
+  constexpr int kChunks = BN / 32;
   const uint32_t sb_u32 = smem_u32(sb);
-  const uint32_t st_row = sb_u32 + row * 128, st_x = (row & 7) << 4;            // phase 1 (own row)
-  const uint32_t ld_a0 = sb_u32 + r0 * 128 + (((2 * cg) ^ (r0 & 7)) << 4);        // phase 2
+  // phase 1: fragment rows (et / 32) * 16 + (et % 32) / 4 (+8), columns 8 q + 2 (et % 4) (+1)
+  const int frow = ((et >> 5) << 4) + ((et & 31) >> 2);
+  const uint32_t st0 = sb_u32 + frow * 128, st1 = st0 + 8 * 128;
+  const uint32_t st_x = (frow & 7) << 4;                 // rows frow and frow + 8 share (row & 7)
+  const uint32_t st_in = (et & 1) << 3;                  // byte offset inside the 16-byte chunk
+  const int st_c = (et & 3) >> 1;                        // 16-byte chunk of the column pair inside 8 columns
+  const uint32_t ld_a0 = sb_u32 + r0 * 128 + (((2 * cg) ^ (r0 & 7)) << 4);   // phase 2
   const uint32_t ld_a1 = sb_u32 + r0 * 128 + (((2 * cg + 1) ^ (r0 & 7)) << 4);
-  // Residual reads come from HBM (~1 us): a group keeps the reads of TWO of its chunks in flight.
-  // Chunks 0 and 1 are issued here, before the accumulator is even complete; chunk jj + 2 is issued
-  // as soon as chunk jj's registers are consumed.  (out may alias residual for in-place accumulation:
-  // every element is read and later written by the same thread, tiles are disjoint.)
-  uint4 rcur[4], rnext[4];
-  auto load_res = [&](uint4 (&dst)[4], int jj) {
-    const int n = n0 + (grp + 2 * jj) * 32 + cg * 8;
-    if (grp + 2 * jj < nchunks && n + 8 <= p.N) {
+  // Residual reads come from HBM: the reads of TWO chunks are kept in flight.  (out may alias
+  // residual for in-place accumulation: every element is read and later written by the same
+  // thread, tiles are disjoint.)
+  uint4 rcur[2], rnext[2];
+  auto load_res = [&](uint4 (&dst)[2], int j) {
+    const int n = n0 + j * 32 + cg * 8;
+    if (j < kChunks && n + 8 <= p.N) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+      for (int i = 0; i < 2; ++i)
         if (valid[i]) dst[i] = *reinterpret_cast<const uint4*>(p.residual + off[i] + n);
     }
   };
@@ -120,22 +126,13 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, int tm, 
     load_res(rcur, 0);
     load_res(rnext, 1);
   }
-  mbar_wait(tfull, tfull_phase);
-  tc_fence_after();
-  const int last_j = ((nchunks - 1 - grp) & ~1) + grp;  // last chunk this group handles
-  if (grp >= nchunks) {  // block_n == 32: group 1 has no chunk, still releases the accumulator
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) release();
-  }
 #pragma unroll 1
-  for (int jj = 0; grp + 2 * jj < nchunks; ++jj) {
-    const int j = grp + 2 * jj;
+  for (int j = 0; j < kChunks; ++j) {
     const int n = n0 + j * 32 + cg * 8;
-    const bool fast = fast_ok && (n0 + j * 32 + 32 <= p.N);  // uniform over the group
-    // bias / row vectors are L2 resident: issued per chunk, ahead of the TMEM load
+    const bool fast = fast_ok && (n0 + j * 32 + 32 <= p.N);  // uniform over the warpgroup
+    // bias / row vectors are L2 resident: issued per chunk, ahead of the staging writes
     float4 bia0 = make_float4(0.f, 0.f, 0.f, 0.f), bia1 = bia0;
-    uint4 rrv[4];
+    uint4 rrv[2];
     if (fast) {
       if (has_bias) {
         bia0 = *reinterpret_cast<const float4*>(p.bias + n);
@@ -143,31 +140,28 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, int tm, 
       }
       if (has_rv) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 2; ++i)
           if (valid[i]) rrv[i] = *reinterpret_cast<const uint4*>(rvp[i] + n);
       }
     }
-    {
-      uint32_t v[32];
-      tmem_ld_32x32(taddr + j * 32, v);
-      tmem_ld_wait();
-      if (j == last_j) {
-        // all TMEM reads of this group for this tile are done: release the accumulator
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) release();
-      }
+    // phase 1 (registers are indexed at compile time: the chunk is selected by predicate)
 #pragma unroll
-      for (int c = 0; c < 8; ++c)
-        sts128(st_row + ((c << 4) ^ st_x), v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
+    for (int jj = 0; jj < kChunks; ++jj) {
+      if (jj != j) continue;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const uint32_t c = (static_cast<uint32_t>(2 * q + st_c) << 4) ^ st_x;
+        const float* a = &acc[16 * jj + 4 * q];
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(st0 + c + st_in), "f"(a[0]), "f"(a[1]) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(st1 + c + st_in), "f"(a[2]), "f"(a[3]) : "memory");
+      }
     }
-    // group-local barrier (ids 1 / 2): staging tile written
-    asm volatile("bar.sync %0, 128;" ::"r"(grp + 1) : "memory");
+    asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");  // staging tile written
     if (fast) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
+      for (int i = 0; i < 2; ++i) {
         if (!valid[i]) continue;
-        // rows r0 + 32 i share (row & 7): same swizzle, 4 KB apart
+        // rows r0 and r0 + 32 share (row & 7): same swizzle, 4 KB apart
         const float4 a0 = lds128(ld_a0 + i * 4096);
         const float4 a1 = lds128(ld_a1 + i * 4096);
         float f[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
@@ -188,14 +182,14 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, int tm, 
       }
       if (has_res) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i) rcur[i] = rnext[i];
-        load_res(rnext, jj + 2);
+        for (int i = 0; i < 2; ++i) rcur[i] = rnext[i];
+        load_res(rnext, j + 2);
       }
     } else if (n < p.N) {
-      gemm_epilogue_rows_generic(p, sb, tm, n, r0, cg, ws);
+      gemm_epilogue_rows_generic(p, sb, m0, n, r0, cg, ws);
     }
-    // staging tile consumed: the group may overwrite it in its next chunk
-    asm volatile("bar.sync %0, 128;" ::"r"(grp + 1) : "memory");
+    // staging tile consumed: the warpgroup may overwrite it in its next chunk
+    asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
   }
 }
 

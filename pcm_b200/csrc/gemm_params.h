@@ -1,4 +1,4 @@
-// Kernel parameter block shared by the 1-CTA and 2-CTA tcgen05 implicit-GEMM kernels.
+// Kernel parameter block of the wgmma implicit-GEMM kernel and its split-K finalize.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -16,7 +16,6 @@ struct KEntry {
 struct alignas(64) GemmParams {
   CUtensorMap a_maps[PCM_MAX_ASRC];
   CUtensorMap b_maps[PCM_MAX_BSRC];
-  CUtensorMap out_map, res_map;  // epilogue v2: [32 col x 32 row] SWIZZLE_64B boxes of out / residual
   KEntry prog[PCM_MAX_PROG];
   int num_prog, lin;
   int M, N;

@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA implicit-GEMM for sm_100a.
+// wgmma / TMA implicit-GEMM for sm_90a.
 //
 //   pcm_gemm  : out[M, N] = alpha * sum_k A[m, k] * Bw[n, k]  (+bias, +per-image row vector,
 //               +residual, optional SiLU).  A is gathered by TMA from up to 6 NHWC bf16 tensors
@@ -11,81 +11,67 @@
 //
 // Replaces the cuDNN / cuBLAS calls that diffusers' UNet2DConditionModel + peft LoRA issue for
 // train_pcm_lora_sd15.py:1192-1198, 1219-1223, 1238-1244, 1263-1268 (forwards) and :1296
-// (backward).  Warp roles: warp0 = TMA producer, warp1 = MMA issuer (+TMEM alloc),
-// warps 2-9 = epilogue.  Two epilogues share the mainloop (gemm_body<EPI2>): v1 = two groups,
-// TMEM -> registers -> smem transposition -> 16-byte coalesced stores (long-K convolutions, fp32 /
-// activation outputs, split-K partial sums); v2 = thread per accumulator row, TMA stores and TMA
-// residual boxes (gemm_epilogue_v2.cuh; default for bf16 outputs with <= 24 K blocks).
+// (backward).  Warpgroup roles: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 =
+// consumers, each owning 64 rows of the 128 x BN output tile: wgmma into registers, then the
+// epilogue from those registers (gemm_epilogue.cuh) while the producer already fills the stages of
+// the next tile.  BN (the N tile, a multiple of 32 up to 256) is a template parameter: it is the N
+// of the wgmma instruction.
 // K-program entries may be restricted to an output-column range (grouped Linear layers sharing
 // their input) or to the leading M tiles (an A source with fewer rows than the output: the LoRA
 // T of the student samples in the merged student + teacher pass).  Weights may be K-blocked
 // ([K/64][N][64], pcm_bsrc.kblocked).  dep_a_src1: late programmatic-dependent-launch wait on the
 // LoRA down-projection, M tiles visited last-to-first.  split-K: ordered workspace slices + finalize.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "host_common.h"
 #include "../../include/pcm_b200.h"
 #include "gemm_params.h"
 #include "gemm_epilogue.cuh"
-#include "gemm_epilogue_v2.cuh"
 
 namespace pcm {
 
-int launch_gemm2(GemmParams& p, const pcm_gemm_desc* d, cudaStream_t stream);  // gemm2_tc.cu
-
-constexpr int kGemmThreads = 320;   // warp0 TMA, warp1 MMA, warps 2-9 epilogue (two groups of 4)
-constexpr int kWgradThreads = 192;
+constexpr int kGemmThreads = 384;   // warpgroup 0 TMA, warpgroups 1-2 wgmma + epilogue
+constexpr int kWgradThreads = 256;  // warpgroup 0 TMA, warpgroup 1 wgmma + reduction
 constexpr int kMaxStages = 8;
-constexpr int kStagingBytes = 2 * 128 * 32 * 4;  // epilogue transposition buffers (fp32)
+constexpr int kStagingBytes = 2 * 64 * 32 * 4;   // epilogue transposition buffers (fp32), one per consumer
 constexpr int kSmemLimit = 227 * 1024 - 512;     // dynamic smem budget (227 KB max minus static)
 
-template <bool EPI2>
-__device__ __forceinline__ void gemm_body(const GemmParams& p) {
+// K blocks of the work item whose output tile starts at rows m0, columns n0 (filtered programs)
+__device__ __forceinline__ int tile_kblocks(const GemmParams& p, int m0, int n0) {
+  int nkb = 0;
+  for (int e = 0; e < p.num_prog; ++e) {
+    const KEntry en = p.prog[e];
+    if ((en.n_hi == 0 || (n0 >= en.n_lo && n0 < en.n_hi)) && (en.m_hi == 0 || m0 < en.m_hi))
+      nkb += en.nchunks;
+  }
+  return nkb;
+}
+
+template <int BN>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ __align__(8) uint64_t rbar[8][2];  // epilogue v2: residual boxes (per warp, 2 in flight)
-  __shared__ uint32_t tmem_base_smem;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int S = p.num_stages;
-  const uint32_t stage_bytes = kATileBytes + p.block_n * 128;
+  constexpr uint32_t stage_bytes = kATileBytes + BN * 128;
   const int num_items = p.tiles_m * p.tiles_n * p.ksplit;
   const int kb_per = (p.num_kblocks + p.ksplit - 1) / p.ksplit;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int i = 0; i < PCM_MAX_ASRC; ++i) tma_prefetch_desc(&p.a_maps[i]);
     for (int i = 0; i < PCM_MAX_BSRC; ++i) tma_prefetch_desc(&p.b_maps[i]);
     for (int i = 0; i < S; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 8);
-    }
-    if (EPI2) {
-      tma_prefetch_desc(&p.out_map);
-      tma_prefetch_desc(&p.res_map);
-      for (int i = 0; i < 8; ++i) {
-        mbar_init(&rbar[i][0], 1);
-        mbar_init(&rbar[i][1], 1);
-      }
+      mbar_init(&empty_bar[i], 2);   // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(&tmem_base_smem, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   // PDL: everything above overlapped the previous kernel's tail.  With a late dependency
   // (dep_a_map >= 0: only the LoRA down-projection T comes from the previous launch, everything else
   // from launches that one has already waited for) the base K blocks start right away and only the
@@ -93,9 +79,10 @@ __device__ __forceinline__ void gemm_body(const GemmParams& p) {
   if (p.dep_a_map < 0) griddep_sync();
   else griddep_launch();
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       bool dep_waited = p.dep_a_map < 0;
@@ -105,7 +92,7 @@ __device__ __forceinline__ void gemm_body(const GemmParams& p) {
         int tm = tile / p.tiles_n;
         const int tn = tile - tm * p.tiles_n;
         if (p.dep_a_map >= 0) tm = p.tiles_m - 1 - tm;  // adapter-free rows first (see dep_a_src1)
-        const int m0 = tm * 128, n0 = tn * p.block_n;
+        const int m0 = tm * 128, n0 = tn * BN;
         int b0 = 0, h0 = 0;
         if (!p.lin) {
           b0 = m0 / p.geoHW;
@@ -147,111 +134,56 @@ __device__ __forceinline__ void gemm_body(const GemmParams& p) {
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(128, p.block_n, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const int ks = item % p.ksplit;
-        int nkb = min(p.num_kblocks, (ks + 1) * kb_per) - ks * kb_per;
-        if (p.filtered) {  // N- or M-ranged entries (ksplit == 1): count the K blocks of this tile
-          int tm = item / p.tiles_n;
-          const int n0 = (item - tm * p.tiles_n) * p.block_n;
-          if (p.dep_a_map >= 0) tm = p.tiles_m - 1 - tm;
-          const int m0 = tm * 128;
-          nkb = 0;
-          for (int e = 0; e < p.num_prog; ++e) {
-            const KEntry en = p.prog[e];
-            if ((en.n_hi == 0 || (n0 >= en.n_lo && n0 < en.n_hi)) && (en.m_hi == 0 || m0 < en.m_hi))
-              nkb += en.nchunks;
-          }
-        }
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-          const uint32_t b_addr = a_addr + kATileBytes;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t ad = umma_desc_sw128(a_addr + k * 32, 16, 1024);
-            const uint64_t bd = umma_desc_sw128(b_addr + k * 32, 16, 1024);
-            umma_f16(d_tmem, ad, bd, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == S) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull_bar[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (EPI2) {
-    // ===================== epilogue v2: thread = row, TMA store / TMA residual =====================
-    const int we = warp - 2;
-    uint8_t* ebuf = smem + S * stage_bytes + we * kEpi2BytesPerWarp;
-    uint64_t* tempty = tempty_bar;
-    gemm_epilogue_v2(p, warp & 3, we >> 2, lane, tmem_base, ebuf, rbar[we], tfull_bar,
-                     [tempty](int acc) { mbar_arrive(&tempty[acc]); });
   } else {
-    // ===================== epilogue =====================
-    // Two phases per 32-column chunk so that global traffic is coalesced:
-    //   1. each thread owns one accumulator row (TMEM lane): TMEM -> registers -> fp32 staging
-    //      tile in shared memory (16-byte chunks XOR-swizzled by row to stay conflict free);
-    //   2. the 128 epilogue threads re-map to (row, 8-column group): 4 neighbouring lanes cover
-    //      64 contiguous output bytes of one row, read residual / bias / row vector, apply the
-    //      activation and store 16 bytes each.
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;
-    const int grp = (warp - 2) >> 2;          // epilogue group 0/1: even / odd 32-column chunks
-    const int et = (threadIdx.x - 64) & 127;  // thread index inside the group
-    const int cg = et & 3;                    // 8-column group inside the 32-column chunk
-    const int r0 = et >> 2;                   // phase-2 rows: r0 + 32 * i
-    float* sb = reinterpret_cast<float*>(smem + S * stage_bytes) + grp * (128 * 32);
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===================== consumers: wgmma mainloop + epilogue =====================
+    regs_alloc<232>();   // 128 x 40 + 256 x 232 <= 64 K registers
+    const int cw = wg - 1;                 // rows cw * 64 .. cw * 64 + 63 of the tile
+    const int et = threadIdx.x & 127;
+    float* sbuf = reinterpret_cast<float*>(smem + S * stage_bytes) + cw * (64 * 32);
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      const int tile = item / p.ksplit;
+      const int tile = item / p.ksplit, ks = item - tile * p.ksplit;
       int tm = tile / p.tiles_n;
       const int tn = tile - tm * p.tiles_n;
       if (p.dep_a_map >= 0) tm = p.tiles_m - 1 - tm;
-      const int n0 = tn * p.block_n;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 256;
-      uint64_t* tempty = &tempty_bar[acc];
-      // split-K: this item's partial sums go to slice (item % ksplit) of the workspace
-      float* ws = p.ws ? p.ws + static_cast<long long>(item - tile * p.ksplit) * p.M * p.N : nullptr;
-      gemm_epilogue_tile(p, tm, n0, taddr, sb, lane, row, grp, cg, r0, &tfull_bar[acc], acc_phase,
-                         [tempty]() { mbar_arrive(tempty); }, ws);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
+      const int n0 = tn * BN;
+      const int nkb = p.filtered ? tile_kblocks(p, tm * 128, n0)   // N- or M-ranged entries (ksplit == 1)
+                                 : min(p.num_kblocks, (ks + 1) * kb_per) - ks * kb_per;
+      if (nkb <= 0) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      }
+      int prev_stage = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * stage_bytes) + cw * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + stage * stage_bytes) + kATileBytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          Wgmma<BN, 0, 0>::mma(acc, wgmma_desc_sw128(a_addr + k * 32, 16, 1024),
+                               wgmma_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_fence_acc(acc);
+        // the previous K block's wgmma are complete: its stage may be refilled
+        wgmma_wait<1>();
+        if (prev_stage >= 0 && et == 0) mbar_arrive(&empty_bar[prev_stage]);
+        prev_stage = stage;
+        if (++stage == S) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (prev_stage >= 0 && et == 0) mbar_arrive(&empty_bar[prev_stage]);
+      // split-K: this item's partial sums go to slice ks of the workspace
+      float* ws = p.ws ? p.ws + static_cast<long long>(ks) * p.M * p.N : nullptr;
+      gemm_epilogue_tile<BN>(p, tm * 128 + cw * 64, n0, acc, sbuf, et, 1 + cw, ws);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-__global__ void __launch_bounds__(kGemmThreads, 1)
-pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<false>(p);
-}
-// same mainloop with the thread-per-row / TMA-store epilogue (gemm_epilogue_v2.cuh)
-__global__ void __launch_bounds__(kGemmThreads, 1)
-pcm_gemm_epi2_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<true>(p);
 }
 
 // split-K finalize: out = act(sum over the ksplit workspace slices, in split order, + bias + rowvec
@@ -337,11 +269,7 @@ pcm_wgrad_kernel(const __grid_constant__ WgradParams p) {
                                              ~static_cast<uintptr_t>(1023));
   __shared__ __align__(8) uint64_t full_bar[kWgStages];
   __shared__ __align__(8) uint64_t empty_bar[kWgStages];
-  __shared__ __align__(8) uint64_t tfull_bar;
-  __shared__ uint32_t tmem_base_smem;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   const int ch0 = blockIdx.x * 128;
   const int tap = blockIdx.y;
   const int per = (p.kblocks_total + p.ksplit - 1) / p.ksplit;
@@ -350,28 +278,20 @@ pcm_wgrad_kernel(const __grid_constant__ WgradParams p) {
   const int nkb = kb_end - kb_begin;
   if (nkb <= 0) return;  // uniform per CTA
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.p_map);
     tma_prefetch_desc(&p.q_map);
     for (int i = 0; i < kWgStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 1);
     }
-    mbar_init(&tfull_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(&tmem_base_smem, 64);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   griddep_sync();  // PDL: everything above overlapped the previous kernel's tail
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (threadIdx.x < 128) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = kb_begin; kb < kb_end; ++kb) {
@@ -398,79 +318,82 @@ pcm_wgrad_kernel(const __grid_constant__ WgradParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(128, 64, 1, 1);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int i = 0; i < nkb; ++i) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t p_addr = smem_u32(smem + stage * kWgStageBytes);
-        const uint32_t q_addr = p_addr + 2 * kATileBytes;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {  // 16 tokens per UMMA
-          const uint64_t ad = umma_desc_sw128(p_addr + k * 2048, kATileBytes, 1024);
-          const uint64_t bd = umma_desc_sw128(q_addr + k * 2048, kATileBytes, 1024);
-          umma_f16(tmem_base, ad, bd, idesc, (i | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[stage]);
-        if (++stage == kWgStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      umma_commit(&tfull_bar);
-    }
   } else {
-    const int q = warp & 3;
-    const int ch = ch0 + q * 32 + lane;
-    mbar_wait(&tfull_bar, 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    float* o = p.out + p.tap_off[tap] + static_cast<long long>(ch) * p.os_row;
+    // two m64 n64 accumulators: channels ch0 .. ch0 + 63 (P tile 0) and ch0 + 64 .. (P tile 1)
+    const int et = threadIdx.x & 127;
+    float acc0[32], acc1[32];
+    int stage = 0;
+    uint32_t phase = 0;
+    int prev_stage = -1;
+    for (int i = 0; i < nkb; ++i) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t p_addr = smem_u32(smem + stage * kWgStageBytes);
+      const uint32_t q_addr = p_addr + 2 * kATileBytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {  // 16 tokens per wgmma
+        const uint64_t bd = wgmma_desc_sw128(q_addr + k * 2048, kATileBytes, 1024);
+        const uint32_t accum = (i | k) != 0 ? 1u : 0u;
+        Wgmma<64, 1, 1>::mma(acc0, wgmma_desc_sw128(p_addr + k * 2048, kATileBytes, 1024), bd, accum);
+        Wgmma<64, 1, 1>::mma(acc1, wgmma_desc_sw128(p_addr + kATileBytes + k * 2048, kATileBytes, 1024), bd,
+                             accum);
+      }
+      wgmma_commit();
+      wgmma_fence_acc(acc0);
+      wgmma_fence_acc(acc1);
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && et == 0) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == kWgStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc0);
+    wgmma_fence_acc(acc1);
     // Deterministic mode: the token splits of one output tile add their partial sums in split
     // order (turnstile on a per-tile semaphore).  Lower blockIdx.z CTAs are dispatched first and
     // never wait on higher ones, so the chain cannot deadlock.
     int* sem = p.sem ? p.sem + (blockIdx.y * gridDim.x + blockIdx.x) : nullptr;
     if (sem) {
-      if (threadIdx.x == 64) {
+      if (et == 0) {
         while (atomicAdd(sem, 0) != static_cast<int>(blockIdx.z)) __nanosleep(64);
         __threadfence();
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");
     }
-    for (int j = 0; j < 64; j += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32(taddr + j, v);
-      tmem_ld_wait();
-      if (ch < p.Cp) {
-        if (p.os_col == 1) {
-          // rank index contiguous (dB layout [n][r]): 16-byte vector reductions, one sector each,
-          // instead of 32 scalar atomics whose lanes are 256 B apart
+    // fragment rows (channels) 16 (et / 32) + (et % 32) / 4 (+8), columns (ranks) 8 q + 2 (et % 4) (+1)
+    const int frow = ((et >> 5) << 4) + ((et & 31) >> 2);
+    const int fcol = 2 * (et & 3);
+    const float* o_base = p.out + p.tap_off[tap];
 #pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            red_add_v4(o + j + i, __uint_as_float(v[i]) * p.alpha, __uint_as_float(v[i + 1]) * p.alpha,
-                       __uint_as_float(v[i + 2]) * p.alpha, __uint_as_float(v[i + 3]) * p.alpha);
-        } else {
+    for (int hf = 0; hf < 2; ++hf) {
+      const float* acc = hf ? acc1 : acc0;
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            atomicAdd(o + static_cast<long long>(j + i) * p.os_col, __uint_as_float(v[i]) * p.alpha);
+      for (int h = 0; h < 2; ++h) {
+        const int ch = ch0 + hf * 64 + frow + 8 * h;
+        if (ch >= p.Cp) continue;
+        float* o = const_cast<float*>(o_base) + static_cast<long long>(ch) * p.os_row;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const int r = 8 * q + fcol;
+          const float v0 = acc[4 * q + 2 * h] * p.alpha, v1 = acc[4 * q + 2 * h + 1] * p.alpha;
+          if (p.os_col == 1) {   // rank index contiguous (dB layout [n][r]): 8-byte vector reductions
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(o + r), "f"(v0), "f"(v1) : "memory");
+          } else {
+            atomicAdd(o + static_cast<long long>(r) * p.os_col, v0);
+            atomicAdd(o + static_cast<long long>(r + 1) * p.os_col, v1);
+          }
         }
       }
     }
     if (sem) {
       __threadfence();
       asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (threadIdx.x == 64)
+      if (et == 0)
         atomicExch(sem, blockIdx.z + 1 == gridDim.z ? 0 : static_cast<int>(blockIdx.z) + 1);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 64);
   }
 }
 
@@ -504,52 +427,19 @@ static int encode_asrc(CUtensorMap* map, const pcm_asrc& a, int lin, int geoW, i
   return encode_tmap(map, a.ptr, 4, dims, strides, box, estr);
 }
 
-static bool epi2_enabled() {
-  static int e = -1;
-  if (e < 0) {
-    const char* s = getenv("PCM_EPI_V2");   // default on; PCM_EPI_V2=0 keeps the two-phase v1 epilogue
-    e = (s != nullptr && s[0] == '0') ? 0 : 1;
+// the wgmma N of the kernel is the N tile of the launch
+typedef void (*GemmKernel)(const GemmParams);
+static GemmKernel gemm_kernel_for(int block_n) {
+  switch (block_n) {
+    case 32: return pcm_gemm_kernel<32>;
+    case 64: return pcm_gemm_kernel<64>;
+    case 96: return pcm_gemm_kernel<96>;
+    case 128: return pcm_gemm_kernel<128>;
+    case 160: return pcm_gemm_kernel<160>;
+    case 192: return pcm_gemm_kernel<192>;
+    case 224: return pcm_gemm_kernel<224>;
+    default: return pcm_gemm_kernel<256>;
   }
-  return e == 1;
-}
-
-// Tensor maps of the epilogue-v2 boxes (32 columns x 32 rows, SWIZZLE_64B) over out / residual.
-// Returns 0 and sets *ok when the row mapping fits such boxes.
-static int encode_epi2_maps(GemmParams& p, const pcm_gemm_desc* d, bool* ok) {
-  *ok = false;
-  const long long W = p.epiW, HW = p.epiHW;
-  cuuint64_t dims[4], strides[3];
-  cuuint32_t box[4] = {32, 32, 1, 1}, estr[4] = {1, 1, 1, 1};
-  if (d->osW % 8 != 0) return 0;
-  if (HW >= (1LL << 30)) {  // plain [M, N] matrix
-    dims[0] = d->N; dims[1] = d->M; dims[2] = 1; dims[3] = 1;
-    strides[0] = d->osW * 2;
-    strides[1] = strides[0] * static_cast<cuuint64_t>(d->M);
-    strides[2] = strides[1];
-  } else {
-    const long long H = HW / W;
-    if (W * H != HW || d->osH % 8 != 0 || d->osB % 8 != 0) return 0;
-    long long bw, bh, bb;
-    if (W >= 32) {
-      if (W % 32 != 0) return 0;
-      bw = 32; bh = 1; bb = 1;
-    } else {
-      if (32 % W != 0) return 0;
-      bw = W;
-      bh = (32 / W) < H ? (32 / W) : H;
-      if (H % bh != 0) return 0;
-      bb = 32 / (bw * bh);
-    }
-    if (bw * bh * bb != 32) return 0;
-    dims[0] = d->N; dims[1] = W; dims[2] = H; dims[3] = (d->M + HW - 1) / HW;
-    strides[0] = d->osW * 2; strides[1] = d->osH * 2; strides[2] = d->osB * 2;
-    box[1] = static_cast<cuuint32_t>(bw); box[2] = static_cast<cuuint32_t>(bh); box[3] = static_cast<cuuint32_t>(bb);
-  }
-  if (int rc = encode_tmap(&p.out_map, d->out, 4, dims, strides, box, estr, 64)) return rc;
-  const void* res = d->residual != nullptr ? d->residual : d->out;
-  if (int rc = encode_tmap(&p.res_map, res, 4, dims, strides, box, estr, 64)) return rc;
-  *ok = true;
-  return 0;
 }
 
 static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
@@ -616,18 +506,7 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
   p.tiles_n = (d->N + d->block_n - 1) / d->block_n;
   p.num_kblocks = nkb;
   const int stage_bytes = kATileBytes + d->block_n * 128;
-  // epilogue v2 (default; PCM_EPI_V2=0 disables): bf16 output, no activation, short K programs (the
-  // epilogue-bound layers; it needs 64 KB of boxes, which the long-K convolutions rather spend on
-  // pipeline stages), row mapping expressible as 32-row TMA boxes
-  bool epi2 = epi2_enabled() && !d->out_fp32 && d->act == 0 && d->N >= 32 && (d->N % 8) == 0 && nkb <= 24 &&
-              !(d->ksplit > 1 && d->splitk_ws != nullptr);
-  p.epiW = d->epiW > 0 ? d->epiW : 1;
-  p.epiHW = d->epiHW > 0 ? d->epiHW : 1;
-  if (epi2) {
-    if (int rc = encode_epi2_maps(p, d, &epi2)) return rc;
-  }
-  const int staging = epi2 ? 8 * kEpi2BytesPerWarp : kStagingBytes;
-  int S = (kSmemLimit - 1024 - staging) / stage_bytes;
+  int S = (kSmemLimit - 1024 - kStagingBytes) / stage_bytes;
   if (S > kMaxStages) S = kMaxStages;
   if (S < 2) return set_error("pcm_gemm: tile too large for shared memory");
   p.num_stages = S;
@@ -654,14 +533,12 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
     p.ksplit = ks;
   }
 
-  const size_t smem = static_cast<size_t>(S) * stage_bytes + staging + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CUDA_TRY(cudaFuncSetAttribute(pcm_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  kSmemLimit));
-    CUDA_TRY(cudaFuncSetAttribute(pcm_gemm_epi2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  kSmemLimit));
-    attr_set = true;
+  const size_t smem = static_cast<size_t>(S) * stage_bytes + kStagingBytes + 1024;
+  const GemmKernel kernel = gemm_kernel_for(d->block_n);
+  static bool attr_set[9] = {};
+  if (!attr_set[d->block_n / 32]) {
+    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    attr_set[d->block_n / 32] = true;
   }
   if (d->dep_a_src1 > 0 && p.ksplit == 1) {  // (split-K: the finalize kernel follows; keep the plain chain)
     if (d->dep_a_src1 > d->num_a) return set_error("pcm_gemm: bad dep_a_src1");
@@ -674,7 +551,7 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
     GemmParams q = p;
     q.ws = reinterpret_cast<float*>(d->splitk_ws);
     q.bias = nullptr; q.rowvec = nullptr; q.residual = nullptr; q.act = 0;
-    CUDA_TRY(launch_pdl(pcm_gemm_kernel, dim3(grid), dim3(kGemmThreads), smem, stream, q));
+    CUDA_TRY(launch_pdl(kernel, dim3(grid), dim3(kGemmThreads), smem, stream, q));
     GemmParams f = p;
     f.ws = q.ws;
     f.alpha = 1.f;
@@ -684,16 +561,7 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
     CUDA_TRY(launch_pdl(splitk_finalize_kernel, dim3(fg), dim3(256), 0, stream, f));
     return 0;
   }
-  if (epi2) {
-    CUDA_TRY(launch_pdl(pcm_gemm_epi2_kernel, dim3(grid), dim3(kGemmThreads), smem, stream, p));
-    CUDA_TRY(cudaGetLastError());
-    return 0;
-  }
-  if (!p.filtered) {
-    const int rc2 = launch_gemm2(p, d, stream);  // 2-CTA kernel for the large layers
-    if (rc2 <= 0) return rc2;
-  }
-  CUDA_TRY(launch_pdl(pcm_gemm_kernel, dim3(grid), dim3(kGemmThreads), smem, stream, p));
+  CUDA_TRY(launch_pdl(kernel, dim3(grid), dim3(kGemmThreads), smem, stream, p));
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -662,7 +662,7 @@ static int gn_launch_cfg(int C, int HW, int B, int* threads, int* ppb, int* nblk
   static int waves = -1;
   if (waves < 0) {
     const char* e = getenv("PCM_GN_WAVES");
-    waves = e ? atoi(e) : 1;   // measured: 1 wave 61 us, 2 waves 66 us, 3 waves 74 us (B=24, C=320 fwd)
+    waves = e ? atoi(e) : 1;   // one wave: fewest partials to merge
     if (waves < 1) waves = 1;
   }
   int target_blocks = (2 * waves * num_sms()) / B;
@@ -689,7 +689,7 @@ static inline size_t gn_ws_need(int B, int nblk, int C, int G) {
 
 // Images per launch pair: the second pass over x (apply / bwd apply) should find it in L2, so a
 // pass may be limited to PCM_GN_CHUNK_MB of input at a time (default 0 = one pass over all images:
-// measured on B200, bs 8 step: chunking at 24 MB costs 2.9 ms / step more than it saves).
+// the bs 8 step has not been re-measured with chunking on the H100).
 static int gn_chunk_images(int B, long long bytes_per_image) {
   static long long limit = -1;
   if (limit < 0) {

@@ -3,7 +3,7 @@
 //   pcm_adamw_clip    : clip_grad_norm_(max_norm) folded into torch.optim.AdamW's update; the
 //                       1/world average of the NCCL sum is folded in too; step counter and lr
 //                       live in device memory so the whole step can sit in one CUDA graph
-//   pcm_lora_refresh  : bf16 operand copies of the LoRA factors in the four layouts the tcgen05
+//   pcm_lora_refresh  : bf16 operand copies of the LoRA factors in the four layouts the wgmma
 //                       GEMMs consume (A, s*B, (s*B)^T, A^T), table driven, one launch
 // Replaces accelerator.clip_grad_norm_ + optimizer.step + zero_grad
 // (train_pcm_lora_sd15.py:1297-1301) and peft's per-op autocast casts of lora_A / lora_B.

@@ -28,7 +28,7 @@ def rank_seed(base_seed, rank):
 
 
 def init_process_group(backend="nccl", device=None):
-    """NVLink-only NCCL defaults for one 8xB200 NVSwitch box; rendezvous from MASTER_* env."""
+    """NVLink-only NCCL defaults for one 8-GPU NVSwitch box (8xH100 SXM); rendezvous from MASTER_* env."""
     if backend == "nccl":
         os.environ.setdefault("NCCL_IB_DISABLE", "1")
         os.environ.setdefault("NCCL_P2P_LEVEL", "NVL")

@@ -4,7 +4,7 @@
          encoder_hidden_states=prompt_embeds.float(), added_cond_kwargs=...).sample      (:1192-1198)
     teacher_unet(...).sample                                                              (:1219-1223)
 
-`UNet2DConditionModel` wraps the B200 network (`pcm_b200.unet.UNetB200`, NHWC bf16 inside) behind
+`UNet2DConditionModel` wraps the CUDA network (`pcm_b200.unet.UNetB200`, NHWC bf16 inside) behind
 diffusers' NCHW signature: CUDA tensors in, `.sample` fp32 NCHW out (accelerate's autocast wrapper
 converts outputs to fp32, SURVEY App. A1).  `use_lora=False` gives the frozen teacher on the SAME
 weights.  The layout change of the 4-channel latents is a torch permute (plumbing, 64 KB / sample);
@@ -44,10 +44,10 @@ class UNet2DConditionModel:
         return [self.net.lora_master] if self.use_lora and self.net.has_lora else []
 
     def enable_gradient_checkpointing(self):
-        """No recompute is needed with 180 GB HBM (SURVEY section 7); accepted for API parity."""
+        """No recompute is needed: the bs 8 SD1.5 step fits an 80 GB H100 without it; accepted for API parity."""
 
     def enable_xformers_memory_efficient_attention(self):
-        """Attention always runs the tcgen05 flash kernels; accepted for API parity."""
+        """Attention always runs the library's flash kernels; accepted for API parity."""
 
     def get_peft_model_state_dict(self):
         return self.net.lora_state_dict()

@@ -65,7 +65,7 @@ _KERNELS_PER_CALL = {"pcm_groupnorm_fwd": 2, "pcm_groupnorm_bwd": 2, "pcm_attn_b
 def num_sms():
     global _NUM_SMS
     if _NUM_SMS is None:
-        _NUM_SMS = 148 if DRY_RUN is not None else L.lib().pcm_num_sms()
+        _NUM_SMS = 132 if DRY_RUN is not None else L.lib().pcm_num_sms()
     return _NUM_SMS
 
 
@@ -115,7 +115,7 @@ def gemm_flops(a_srcs, prog, M, N, lin, geo):
 def gemm(a_srcs, b_srcs, prog, *, lin, M, N, out, geo=(1, 1), bias=None, rowvec=None,
          residual=None, out_strides=None, epi=None, alpha=1.0, act=0, round_bf16=False,
          block_n=None, ksplit=None, dep_a_src=None, splitk_ws=None):
-    """Launch the tcgen05 implicit GEMM.  prog: list of (a_src, b_src, dw, dh, nchunks, a_c0, b_k0
+    """Launch the wgmma implicit GEMM.  prog: list of (a_src, b_src, dw, dh, nchunks, a_c0, b_k0
     [, n_lo, n_hi]); an entry with n_hi > 0 only feeds output columns [n_lo, n_hi).
 
     dep_a_src: index of the A source that the launch issued IMMEDIATELY before this one produced (the

@@ -1,4 +1,4 @@
-"""One PCM-LoRA distillation iteration on the B200 path: the body of the reference loop
+"""One PCM-LoRA distillation iteration on the CUDA path: the body of the reference loop
 train_pcm_lora_sd15.py:1139-1301 (noise / phase bookkeeping, student forward, teacher CFG DDIM
 step, target forward, Huber loss, backward, gradient all-reduce, clip + AdamW) as a fixed sequence
 of C-ABI kernel launches, capturable in ONE CUDA graph (no host sync inside; `index`, `w`,
@@ -259,7 +259,7 @@ class PCMTrainStep:
             # ONE graph for the whole iteration.  Data parallel default: graph(forward + backward) ->
             # eager NCCL all-reduce -> graph(optimiser).  PCM_NCCL_IN_GRAPH=1 (experimental) captures the
             # bucketed, backward-overlapped all-reduces inside the single graph: it steps correctly on 2
-            # GPUs (measured 78.6 vs 78.5 ms/step) but process-group teardown hung while the graph was
+            # GPUs but process-group teardown hung while the graph was
             # alive, so it is not the default; drop `self.graph` before destroy_process_group().
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""`train_pcm_lora_sd15` entry point on the B200 path.
+"""`train_pcm_lora_sd15` entry point on the CUDA path.
 
 Keeps the reference script's command line (flag names / defaults of
-/root/reference/code/text_to_image_sd15/train_pcm_lora_sd15.py:381-735) so existing launch recipes
+code/text_to_image_sd15/train_pcm_lora_sd15.py:381-735) so existing launch recipes
 (`train_pcm_lora_sd15.sh`) keep working; the per-iteration hot path runs through libpcm_b200.so
 (PCMTrainStep).  What is NOT here (out of scope, SURVEY.md section 8): the image dataset, VAE and CLIP
 encoders, validation image logging, hub upload.  Inputs to the step are therefore either
@@ -33,7 +33,7 @@ from .step import PCMTrainStep
 
 
 def parse_args(argv=None, extra=None):
-    p = argparse.ArgumentParser(description="PCM-LoRA distillation on B200")
+    p = argparse.ArgumentParser(description="PCM-LoRA distillation on H100")
     if extra is not None:
         extra(p)
     # ---- flags of the reference script, verbatim names / defaults ----
@@ -109,9 +109,9 @@ def parse_args(argv=None, extra=None):
     if args.gradient_accumulation_steps != 1:
         raise ValueError("pcm_b200 runs one optimiser step per iteration (all reference recipes use 1)")
     if args.use_8bit_adam:
-        raise ValueError("--use_8bit_adam (bitsandbytes) is not provided: 180 GB HBM holds fp32 AdamW state")
+        raise ValueError("--use_8bit_adam (bitsandbytes) is not provided: an 80 GB H100 holds the fp32 AdamW state of the LoRA factors (0.54 GB)")
     if args.mixed_precision == "no":
-        raise ValueError("--mixed_precision no (fp32 compute) is not provided: the tcgen05 path computes with "
+        raise ValueError("--mixed_precision no (fp32 compute) is not provided: the CUDA path computes with "
                          "bf16 operands and fp32 accumulation; use bf16")
     if args.mixed_precision == "fp16":
         # every shipped recipe passes fp16 (train_pcm_lora_sd15.sh:9).  fp16 and bf16 run on the same

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""`train_pcm_lora_sdxl_adv` entry point on the B200 path (SURVEY section 8f-2).
+"""`train_pcm_lora_sdxl_adv` entry point on the CUDA path (SURVEY section 8f-2).
 
-Same command line as /root/reference/code/text_to_image_sdxl/train_pcm_lora_sdxl_adv.py (the SD1.5
+Same command line as code/text_to_image_sdxl/train_pcm_lora_sdxl_adv.py (the SD1.5
 flags plus --adv_weight, --adv_lr, --train_shards_path_or_url, --use_fix_crop_and_size) driving the
 SDXL UNet (3 levels, transformer depth 1 / 2 / 10, 64-wide heads, 2048-d context, Linear projections,
 `added_cond_kwargs` text_time embedding, zero unconditional embeddings).  The consistency-distillation
@@ -25,7 +25,7 @@ def parse_args(argv=None):
     args = base.parse_args(argv, extra=_extra)
     if args.adv_weight != 0:
         raise ValueError("the adversarial consistency loss (discriminator_sdxl.Discriminator) is not implemented "
-                         "on the B200 path: pass --adv_weight 0 to run the consistency-distillation step alone")
+                         "on the CUDA path: pass --adv_weight 0 to run the consistency-distillation step alone")
     args._base_cfg = config.SDXL
     return args
 

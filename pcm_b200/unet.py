@@ -1,4 +1,4 @@
-"""B200-native SD1.5 UNet (student / target with fused LoRA, frozen teacher) -- host orchestration.
+"""H100 (sm_90a) SD1.5 UNet (student / target with fused LoRA, frozen teacher) -- host orchestration.
 
 Python only sequences C-ABI kernel launches (pcm_b200.ops); every FLOP runs in libpcm_b200.so.
 Mirrors the call `unet(sample, timestep, encoder_hidden_states=...).sample` of diffusers'
@@ -6,7 +6,7 @@ UNet2DConditionModel wrapped by peft (train_pcm_lora_sd15.py:1192-1198 student, 
 teacher, :1263-1268 target) and its autograd backward (:1296), with:
   * activations NHWC bf16, one rounding per materialised tensor (bf16 autocast semantics);
   * LoRA unmerged: T = A(x) as a 64-wide GEMM, then s*B*T enters the base GEMM as one extra
-    64-wide K block (same TMEM accumulator), so `base(x) + B(A(x)) * scaling` is one kernel;
+    64-wide K block (same wgmma accumulator), so `base(x) + B(A(x)) * scaling` is one kernel;
   * skip concats never materialised (two K segments / two GroupNorm sources);
   * backward = explicit tape: dgrad through every layer, wgrad for LoRA factors only.
 Parameters use diffusers state-dict names; LoRA factors live in ONE flat fp32 buffer
@@ -345,8 +345,8 @@ class UNetB200:
     def _block_weights(self):
         """Store every frozen GEMM weight K-blocked ([K/64][N][64], pcm_bsrc.kblocked): the operand tile of
         a K block becomes one contiguous run in HBM.  Matters for the small-M layers (8x8 / 16x16 levels,
-        target pass), which stream their weights once per launch: 1.2 TB/s with row-major tiles (N separate
-        128-byte segments K*2 bytes apart).  PCM_KBLOCK=0 keeps the row-major layout."""
+        target pass), which stream their weights once per launch: a row-major tile is N separate
+        128-byte segments K*2 bytes apart.  PCM_KBLOCK=0 keeps the row-major layout."""
         import os as _os
         if _os.environ.get("PCM_KBLOCK", "1") == "0":
             return

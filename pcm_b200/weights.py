@@ -1,4 +1,4 @@
-"""Weight sources for the B200 UNet: seeded synthetic initialisation (no pretrained checkpoint is
+"""Weight sources for the UNet: seeded synthetic initialisation (no pretrained checkpoint is
 available offline) and state-dict helpers using diffusers / peft key names, so a real
 `runwayml/stable-diffusion-v1-5` UNet state dict can be dropped in unchanged
 (train_pcm_lora_sd15.py:840-852, 866-885)."""

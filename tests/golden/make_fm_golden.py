@@ -3,7 +3,7 @@
 reference classes verbatim (AST-extracted from the read-only tree; the diffusers mixins they inherit
 from are replaced by empty stand-ins, which only provide `.config`):
 
-    EulerSolver                   /root/reference/code/text_to_image_sd3/train_pcm_lora_sd3.py:160-226
+    EulerSolver                   $PCM_REFERENCE/code/text_to_image_sd3/train_pcm_lora_sd3.py:160-226
     PCMFMDeterministicScheduler   .../pcm_fm_deterministic_scheduler.py:35-242
     PCMFMStochasticScheduler      .../pcm_fm_stochastic_scheduler.py:35-243
 
@@ -16,7 +16,8 @@ import types
 import numpy as np
 import torch
 
-REF = "/root/reference/code/text_to_image_sd3"
+# a checkout of G-U-N/Phased-Consistency-Model (read only), given by PCM_REFERENCE
+REF = os.path.join(os.environ["PCM_REFERENCE"], "code/text_to_image_sd3")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "fm_math.pt")
 
 

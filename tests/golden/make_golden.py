@@ -3,7 +3,7 @@
 The reference training script cannot be imported (diffusers / peft / accelerate are not installed),
 but its PCM math is plain torch + numpy: this script AST-extracts `DDIMSolver`, `predicted_origin`,
 `extract_into_tensor`, `append_dims`, `scalings_for_boundary_conditions_{target,online}` from
-/root/reference/code/text_to_image_sd15/train_pcm_lora_sd15.py and `add_noise` / `noise_travel`
+$PCM_REFERENCE/code/text_to_image_sd15/train_pcm_lora_sd15.py and `add_noise` / `noise_travel`
 from scheduling_ddpm_modified.py, executes them verbatim on seeded inputs, and stores inputs and
 outputs.  Run here (the reference tree is not available on the GPU box); the fixture is committed.
 
@@ -17,7 +17,8 @@ import types
 import numpy as np
 import torch
 
-REF = "/root/reference/code/text_to_image_sd15"
+# a checkout of G-U-N/Phased-Consistency-Model (read only), given by PCM_REFERENCE
+REF = os.path.join(os.environ["PCM_REFERENCE"], "code/text_to_image_sd15")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

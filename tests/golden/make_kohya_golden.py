@@ -14,7 +14,8 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = "/root/reference/code/text_to_image_sd15/train_pcm_lora_sd15.py"
+# a checkout of G-U-N/Phased-Consistency-Model (read only), given by PCM_REFERENCE
+REF = os.path.join(os.environ["PCM_REFERENCE"], "code/text_to_image_sd15/train_pcm_lora_sd15.py")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "kohya_keys.json")
 
 

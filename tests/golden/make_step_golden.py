@@ -10,6 +10,8 @@ without CUDA, T15:1139-1293 run in fp32) and `bf16` (emulate_bf16=True: weights 
 reference materialises under bf16 autocast rounded to bf16).  Seeded synthetic weights
 (unet_ref.init_params(SD15, 0), LoRA B ~ N(0, 0.02)) and inputs (pcm_ref.make_batch(seed=0)); a
 checksum of the weights is stored so the GPU test can verify it regenerated the same parameters.
+Tensors larger than SAMPLE elements (config 2) are stored as a fixed, seeded sample of flat NCHW
+positions (`sample_idx`, the same positions for every tensor) so that each file stays well under 1 MB.
 
     python tests/golden/make_step_golden.py [1] [2]      ->  tests/golden/step_config{1,2}.pt
 """
@@ -25,6 +27,24 @@ sys.path.insert(0, ROOT)
 from oracle import pcm_ref, unet_ref  # noqa: E402
 
 CONFIGS = {1: dict(B=1, hw=32, multiphase=2), 2: dict(B=8, hw=64, multiphase=4)}
+SAMPLE = 16384
+TENSORS = ("eps_student", "x_prev", "model_pred", "target", "noisy")
+
+
+def sample_tensors(out):
+    """Replace every stored latent-shaped tensor by its values at `sample_idx` when it has more than
+    SAMPLE elements (seeded positions, sorted)."""
+    n = out["bf16"]["x_prev"].numel()
+    if n <= SAMPLE:
+        return out
+    g = torch.Generator().manual_seed(20240)
+    idx = torch.randperm(n, generator=g)[:SAMPLE].sort().values
+    out["sample_idx"] = idx.to(torch.int32)
+    for mode in ("fp32", "bf16"):
+        for k in TENSORS:
+            if k in out[mode]:
+                out[mode][k] = out[mode][k].reshape(-1)[idx].clone()
+    return out
 
 
 def param_checksum(P):
@@ -55,7 +75,7 @@ def main():
                              end_timesteps=r["end_timesteps"])
             if emu:
                 out[mode]["noisy"] = r["noisy"].float()     # bit-exact target of pcm_add_noise
-        torch.save(out, os.path.join(ROOT, "tests", "golden", f"step_config{c}.pt"))
+        torch.save(sample_tensors(out), os.path.join(ROOT, "tests", "golden", f"step_config{c}.pt"))
 
 
 if __name__ == "__main__":

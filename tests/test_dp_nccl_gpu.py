@@ -3,7 +3,7 @@ all-reduce(SUM) overlapped with the backward pass, 1/world and the clip folded i
 two ranks with DIFFERENT batches must end with bit-identical LoRA parameters, equal to a single
 process applying clip_grad_norm_ + AdamW to the MEAN of the two local gradients - what DDP +
 accelerate do in the reference (train_pcm_lora_sd15.py:1034, 1296-1301).  Needs 2 GPUs
-(`gpurun --gpus 2 -- python -m pytest tests/test_dp_nccl_gpu.py -m gpu`); skipped otherwise."""
+(`python -m pytest tests/test_dp_nccl_gpu.py -m gpu` on a 2-GPU machine); skipped otherwise."""
 import os
 import socket
 

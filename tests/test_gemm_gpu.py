@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 implicit GEMM (pcm_gemm / pcm_wgrad) against plain PyTorch fp32 ops
+"""Parity of the wgmma implicit GEMM (pcm_gemm / pcm_wgrad) against plain PyTorch fp32 ops
 (F.linear / F.conv2d on bf16-rounded inputs).  Tolerance: outputs are bf16 (rel 2^-9 rounding),
 accumulation fp32 -> |err| <= 1e-2 * max|ref| elementwise and mean error <= 2e-3 * rms(ref)."""
 import pytest

@@ -26,7 +26,7 @@ pytestmark = pytest.mark.gpu
 BF = torch.bfloat16
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
-# measured on B200 (see DESIGN.md section 4); asserted at <= ~2x the measured error.
+# see DESIGN.md section 4 for why the fp32-oracle bounds sit above the bf16 ones.
 # Config 2 (N = 131072 loss terms): 2.7e-4 and 7.8e-5 on two builds -> 2e-3 (north-star 1e-3 met).
 # Config 1 (N = 4096 loss terms only): the loss is a mean of |model_pred - target| over few, noisy terms;
 # two builds with IDENTICAL tensor accuracy (rel-L2 eps 8.29e-3 both) measured 3.0e-3 and 6.8e-3 -> 1.5e-2.
@@ -46,6 +46,13 @@ def _nchw(x):
 
 def _rel(a, b):
     return ((a.double() - b.double()).norm() / (b.double().norm() + 1e-30)).item()
+
+
+def _at(g, x):
+    """x (NCHW, on the CPU) at the positions the golden file stores: all of them, or the fixed sample
+    `sample_idx` of flat positions (config 2)."""
+    idx = g.get("sample_idx")
+    return x if idx is None else x.reshape(-1)[idx.long()]
 
 
 _CACHE = {}
@@ -95,10 +102,10 @@ def _report(tag, c, st, g):
         r = g[mode]
         rows[mode] = dict(
             loss=abs(st.loss.item() - r["loss"].item()) / abs(r["loss"].item()),
-            eps_student=_rel(_nchw(st.debug["eps_student"]).cpu(), r["eps_student"]),
-            x_prev=_rel(_nchw(st.x_prev).cpu(), r["x_prev"]),
-            model_pred=_rel(_nchw(st.model_pred).cpu(), r["model_pred"]),
-            target=_rel(_nchw(st.target).cpu(), r["target"]))
+            eps_student=_rel(_at(g, _nchw(st.debug["eps_student"]).cpu()), r["eps_student"]),
+            x_prev=_rel(_at(g, _nchw(st.x_prev).cpu()), r["x_prev"]),
+            model_pred=_rel(_at(g, _nchw(st.model_pred).cpu()), r["model_pred"]),
+            target=_rel(_at(g, _nchw(st.target).cpu()), r["target"]))
         print(f"[parity config {c} {tag}] vs {mode} oracle: loss {st.loss.item():.8f} (oracle "
               f"{r['loss'].item():.8f}) rel {rows[mode]['loss']:.3e} | rel-L2 eps {rows[mode]['eps_student']:.3e} "
               f"x_prev {rows[mode]['x_prev']:.3e} model_pred {rows[mode]['model_pred']:.3e} "
@@ -111,7 +118,7 @@ def _check(c, st, g, rows):
     assert torch.equal(st.start_t.cpu(), r["start_timesteps"])
     assert torch.equal(st.t.cpu(), r["timesteps"])
     assert torch.equal(st.end_t.cpu(), r["end_timesteps"])
-    assert torch.equal(_nchw(st.noisy).cpu(), r["noisy"])            # add_noise is bit-exact
+    assert torch.equal(_at(g, _nchw(st.noisy).cpu()), r["noisy"])   # add_noise is bit-exact
     assert rows["bf16"]["loss"] <= LOSS_TOL_BF16[c], rows
     assert rows["fp32"]["loss"] <= LOSS_TOL_FP32[c], rows
     for k in ("eps_student", "x_prev", "model_pred", "target"):

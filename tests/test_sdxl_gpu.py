@@ -1,4 +1,4 @@
-"""SDXL-shaped UNet on the B200 path (SURVEY section 8f-2, BASELINE config 4 without the adversarial
+"""SDXL-shaped UNet on the CUDA path (SURVEY section 8f-2, BASELINE config 4 without the adversarial
 term): three levels (DownBlock2D, 2 x CrossAttnDownBlock2D), transformer depth > 1, 64-wide heads,
 Linear proj_in / proj_out, `added_cond_kwargs` (text_time embedding), zero unconditional embeddings,
 40 DDIM steps - train_pcm_lora_sdxl_adv.py:307-366, 1094-1133, 1215-1221.  Parity against the oracle

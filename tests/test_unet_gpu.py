@@ -1,4 +1,4 @@
-"""Whole-network and whole-step parity of the B200 path against the CPU oracle (oracle/unet_ref.py,
+"""Whole-network and whole-step parity of the CUDA path against the CPU oracle (oracle/unet_ref.py,
 oracle/pcm_ref.py) on identical seeded weights and inputs.
 
 Tolerances: the CUDA path computes in bf16 with fp32 accumulation; the oracle is run in its
