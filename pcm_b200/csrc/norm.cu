@@ -6,7 +6,6 @@
 // Transformer2DModel and BasicTransformerBlock (called from train_pcm_lora_sd15.py:1192-1198,
 // 1219-1244, 1263-1268) and their autograd backward (:1296).  GroupNorm reads an optional second
 // source so the up-block skip concat torch.cat([h, res], dim=1) is never materialised twice.
-#include <stdlib.h>
 #include "common.cuh"
 #include "host_common.h"
 #include "../../include/pcm_b200.h"
@@ -655,17 +654,11 @@ static int gn_launch_cfg(int C, int HW, int B, int* threads, int* ppb, int* nblk
   int ny = 512 / nvec;      // ny * nvec <= 512 threads  =>  ny * C <= 4096 staged floats
   if (ny < 1) ny = 1;
   *threads = nvec * ny;
-  // ONE wave of blocks at two resident blocks per SM (all four kernels are built for <= 64 registers;
-  // PCM_GN_WAVES overrides):
+  // ONE wave of blocks at two resident blocks per SM (all four kernels are built for <= 64 registers),
+  // which also keeps the number of partials to merge small:
   // the total block count is at most 2 x 2 x SMs, so there is no third, nearly empty wave (ncu showed
   // the SMs idle for 36 % of the kernel with 600 blocks on 296 slots)
-  static int waves = -1;
-  if (waves < 0) {
-    const char* e = getenv("PCM_GN_WAVES");
-    waves = e ? atoi(e) : 1;   // one wave: fewest partials to merge
-    if (waves < 1) waves = 1;
-  }
-  int target_blocks = (2 * waves * num_sms()) / B;
+  int target_blocks = (2 * num_sms()) / B;
   if (target_blocks < 1) target_blocks = 1;
   int p = (HW + target_blocks - 1) / target_blocks;
   if (p < ny * 4) p = ny * 4;
@@ -687,24 +680,10 @@ static inline size_t gn_ws_need(int B, int nblk, int C, int G) {
          sizeof(float) * static_cast<size_t>(B) * nblk * (2 * G + C);
 }
 
-// Images per launch pair: the second pass over x (apply / bwd apply) should find it in L2, so a
-// pass may be limited to PCM_GN_CHUNK_MB of input at a time (default 0 = one pass over all images:
-// the bs 8 step has not been re-measured with chunking on the H100).
-static int gn_chunk_images(int B, long long bytes_per_image) {
-  static long long limit = -1;
-  if (limit < 0) {
-    const char* e = getenv("PCM_GN_CHUNK_MB");
-    limit = (e ? atoll(e) : 0) * 1024 * 1024;
-  }
-  if (limit <= 0) return B;
-  long long n = limit / (bytes_per_image > 0 ? bytes_per_image : 1);
-  if (n < 1) n = 1;
-  return n > B ? B : static_cast<int>(n);
-}
-
 extern "C" int64_t pcm_groupnorm_ws_bytes(int B, int HW, int C, int G) {
   int threads, ppb, nblk;
-  // the per-chunk launch never uses more blocks per image than a single-image launch would
+  // an upper bound: a launch over B images never uses more blocks per image than a single-image
+  // launch would
   if (gn_launch_cfg(C, HW, 1, &threads, &ppb, &nblk)) return -1;
   return static_cast<int64_t>(gn_ws_need(B, nblk, C, G));
 }
@@ -722,21 +701,14 @@ extern "C" int pcm_groupnorm_fwd(const void* x1_, const void* x2_, int C1, int C
   bf16* out = reinterpret_cast<bf16*>(out_);
   unsigned* counters = reinterpret_cast<unsigned*>(ws);
   float* part = reinterpret_cast<float*>(counters + 3 * kGnMaxB);
-  const int cb = gn_chunk_images(B, 2LL * HW * C);
-  for (int b0 = 0; b0 < B; b0 += cb) {
-    const int nb = B - b0 < cb ? B - b0 : cb;
-    int threads, ppb, nblk;
-    if (int rc = gn_launch_cfg(C, HW, nb, &threads, &ppb, &nblk)) return rc;
-    if (ws == nullptr || static_cast<size_t>(ws_bytes) < gn_ws_need(nb, nblk, C, G))
-      return set_error("groupnorm: workspace too small (see pcm_groupnorm_ws_bytes)");
-    const long long o1 = static_cast<long long>(b0) * HW * C1, o2 = static_cast<long long>(b0) * HW * C2;
-    const bf16* y2 = x2 ? x2 + o2 : nullptr;
-    CUDA_TRY(launch_pdl(gn_stats_kernel, dim3(nblk, nb), dim3(threads), 0, stream, x1 + o1, y2, C1, C2,
-                        HW, G, ppb, eps, part, counters + b0, stats + 2 * b0 * G));
-    CUDA_TRY(launch_pdl(gn_apply_kernel, dim3(nblk, nb), dim3(threads), 0, stream, x1 + o1, y2, C1, C2,
-                        HW, G, ppb, static_cast<const float*>(stats + 2 * b0 * G), gamma, beta, silu,
-                        out + static_cast<long long>(b0) * HW * C));
-  }
+  int threads, ppb, nblk;
+  if (int rc = gn_launch_cfg(C, HW, B, &threads, &ppb, &nblk)) return rc;
+  if (ws == nullptr || static_cast<size_t>(ws_bytes) < gn_ws_need(B, nblk, C, G))
+    return set_error("groupnorm: workspace too small (see pcm_groupnorm_ws_bytes)");
+  CUDA_TRY(launch_pdl(gn_stats_kernel, dim3(nblk, B), dim3(threads), 0, stream, x1, x2, C1, C2,
+                      HW, G, ppb, eps, part, counters, stats));
+  CUDA_TRY(launch_pdl(gn_apply_kernel, dim3(nblk, B), dim3(threads), 0, stream, x1, x2, C1, C2,
+                      HW, G, ppb, static_cast<const float*>(stats), gamma, beta, silu, out));
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -758,28 +730,16 @@ extern "C" int pcm_groupnorm_bwd(const void* dy_, const void* x1_, const void* x
   bf16* dx2 = reinterpret_cast<bf16*>(dx2_);
   unsigned* counters = reinterpret_cast<unsigned*>(ws);
   float* part = reinterpret_cast<float*>(counters + 3 * kGnMaxB);
-  // dy + x (+ add) are read twice: chunk on their combined footprint
-  const int cb = gn_chunk_images(B, (add ? 6LL : 4LL) * HW * C);
-  for (int b0 = 0; b0 < B; b0 += cb) {
-    const int nb = B - b0 < cb ? B - b0 : cb;
-    int threads, ppb, nblk;
-    if (int rc = gn_launch_cfg(C, HW, nb, &threads, &ppb, &nblk)) return rc;
-    if (ws == nullptr || static_cast<size_t>(ws_bytes) < gn_ws_need(nb, nblk, C, G))
-      return set_error("groupnorm: workspace too small (see pcm_groupnorm_ws_bytes)");
-    const long long o = static_cast<long long>(b0) * HW * C;
-    const long long o1 = static_cast<long long>(b0) * HW * C1, o2 = static_cast<long long>(b0) * HW * C2;
-    const bf16* y2 = x2 ? x2 + o2 : nullptr;
-    float* cpart = part + static_cast<size_t>(nb) * nblk * 2 * G;
-    CUDA_TRY(launch_pdl(gn_bwd_stats_kernel, dim3(nblk, nb), dim3(threads), 0, stream, dy + o, x1 + o1,
-                        y2, C1, C2, HW, G, ppb, stats + 2 * b0 * G, gamma, beta, silu, part,
-                        counters + kGnMaxB + b0, red + 2 * b0 * G));
-    CUDA_TRY(launch_pdl(gn_bwd_apply_kernel, dim3(nblk, nb), dim3(threads), 0, stream, dy + o, x1 + o1,
-                        y2, C1, C2, HW, G, ppb, stats + 2 * b0 * G,
-                        static_cast<const float*>(red + 2 * b0 * G), gamma, beta, silu,
-                        add ? add + o : nullptr, dx1 + o1, dx2 ? dx2 + o2 : nullptr,
-                        colsum ? colsum + static_cast<long long>(b0) * C : nullptr, cpart,
-                        counters + 2 * kGnMaxB + b0));
-  }
+  int threads, ppb, nblk;
+  if (int rc = gn_launch_cfg(C, HW, B, &threads, &ppb, &nblk)) return rc;
+  if (ws == nullptr || static_cast<size_t>(ws_bytes) < gn_ws_need(B, nblk, C, G))
+    return set_error("groupnorm: workspace too small (see pcm_groupnorm_ws_bytes)");
+  float* cpart = part + static_cast<size_t>(B) * nblk * 2 * G;
+  CUDA_TRY(launch_pdl(gn_bwd_stats_kernel, dim3(nblk, B), dim3(threads), 0, stream, dy, x1, x2, C1, C2,
+                      HW, G, ppb, stats, gamma, beta, silu, part, counters + kGnMaxB, red));
+  CUDA_TRY(launch_pdl(gn_bwd_apply_kernel, dim3(nblk, B), dim3(threads), 0, stream, dy, x1, x2, C1, C2,
+                      HW, G, ppb, stats, static_cast<const float*>(red), gamma, beta, silu, add, dx1, dx2,
+                      colsum, cpart, counters + 2 * kGnMaxB));
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -792,12 +752,7 @@ extern "C" int pcm_layernorm_fwd(const void* x, int M, int C, const float* gamma
   const int wpb = 8, lpr = ln_lpr(C);
   const int rows_per_block = wpb * (32 / lpr);
   int grid = (M + rows_per_block - 1) / rows_per_block;
-  static int persist = -1;   // PCM_LN_PERSIST=0: one block per 8 x RPW rows (round-1 behaviour)
-  if (persist < 0) {
-    const char* e = getenv("PCM_LN_PERSIST");
-    persist = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
-  if (persist && grid > 4 * num_sms()) grid = 4 * num_sms();   // 4 resident blocks per SM, grid-stride
+  if (grid > 4 * num_sms()) grid = 4 * num_sms();   // 4 resident blocks per SM, grid-stride
   const bf16* xp = reinterpret_cast<const bf16*>(x);
   bf16* op = reinterpret_cast<bf16*>(out);
   if (lpr == 8) CUDA_TRY(launch_pdl(ln_fwd_kernel<8>, dim3(grid), dim3(wpb * 32), 0, stream, xp, M, C, gamma, beta, eps, op, stats));

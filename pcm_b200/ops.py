@@ -51,8 +51,6 @@ def bsrc(w):
 
 
 _NUM_SMS = None
-# late programmatic-dependent-launch wait of a GEMM on its LoRA down-projection (PCM_LATE_WAIT=0: off)
-LATE_WAIT = os.environ.get("PCM_LATE_WAIT", "1") != "0"
 # kernel-launch accounting (bench.py `gpu_launches`) and optional per-launch GEMM profiling
 LAUNCHES = {"count": 0}
 PROFILE = None  # list of (start_event, end_event, flops) when enabled
@@ -173,7 +171,7 @@ def gemm(a_srcs, b_srcs, prog, *, lin, M, N, out, geo=(1, 1), bias=None, rowvec=
     d.epiW, d.epiHW = epi
     d.alpha = alpha
     d.act = act
-    d.dep_a_src1 = 0 if (dep_a_src is None or not LATE_WAIT) else dep_a_src + 1
+    d.dep_a_src1 = 0 if dep_a_src is None else dep_a_src + 1
     LAUNCHES["count"] += 1
     if DRY_RUN is not None:
         DRY_RUN.append(("gemm", dict(M=M, N=N, K=64 * sum(e[4] for e in prog), bn=d.block_n, lin=int(lin),
@@ -202,7 +200,6 @@ TAPS3 = [(kw - 1, kh - 1) for kh in range(3) for kw in range(3)]  # (dw, dh), ta
 # a wgrad tile then accumulate in split order
 WGRAD_SEM = None
 _DET = os.environ.get("PCM_DETERMINISTIC", "0") == "1"
-_SKIP_WGRAD = os.environ.get("PCM_DEBUG_SKIP_WGRAD", "0") == "1"
 
 
 def deterministic(on, device=None):
@@ -238,8 +235,6 @@ def wgrad(p_src, q_src, out, *, lin, M, geo=(1, 1), taps=((0, 0),), tap_off=(0,)
     LAUNCHES["count"] += 1
     if DRY_RUN is not None:
         DRY_RUN.append(("wgrad", dict(M=M, Cp=p_src.C, taps=len(taps))))
-        return out
-    if _SKIP_WGRAD:     # measurement aid only (PCM_DEBUG_SKIP_WGRAD=1): how much of the step the wgrads cost
         return out
     L.check(L.lib().pcm_wgrad(C.byref(d), _stream()), "pcm_wgrad")
     return out

@@ -109,7 +109,6 @@ class PCMTrainStep:
         if self.addc:
             self.in_text3 = torch.zeros(3 * B, cfg.text_embed_dim, device=device, dtype=BF16)
             self.in_time_ids3 = torch.zeros(3 * B, cfg.num_time_ids, **i64)
-        self.merged = os.environ.get("PCM_MERGE_PASSES", "1") != "0"
         # data parallel: overlap the gradient all-reduce with the backward pass (PCM_DP_OVERLAP=0: one
         # flat all-reduce after the backward)
         self._overlap = os.environ.get("PCM_DP_OVERLAP", "1") != "0"
@@ -138,24 +137,13 @@ class PCMTrainStep:
 
         def added(lo, hi):
             return (self.in_text3[lo:hi], self.in_time_ids3[lo:hi]) if self.addc else None
-        if self.merged:
-            # one pass: [student | teacher cond | teacher uncond]; LoRA only on the student samples
-            eps_all = u.forward(self.noisy3[:nb * B], self.start_t3[:nb * B],
-                                self.in_ctx3 if nb == 3 else self.in_ctx3[:2 * B * 77],
-                                lora=True, save=True, lora_batch=B, added_cond=added(0, nb * B))
-            kv = u.last_ctx_kv
-            eps_s, eps_c = eps_all[:B], eps_all[B:2 * B]
-            eps_u = eps_all[2 * B:] if nb == 3 else eps_c
-        else:
-            eps_s = u.forward(self.noisy, self.start_t, self.in_prompt, lora=True, save=True, added_cond=added(0, B))
-            kv = u.last_ctx_kv
-            if self.apply_cfg:
-                eps_cu = u.forward(self.noisy3[B:], self.start_t3[B:], self.in_ctx3[B * 77:], lora=False,
-                                   added_cond=added(B, 3 * B))
-                eps_c, eps_u = eps_cu[:B], eps_cu[B:]
-            else:
-                eps_c = u.forward(self.noisy, self.start_t, self.in_prompt, lora=False, added_cond=added(0, B))
-                eps_u = eps_c
+        # one pass: [student | teacher cond | teacher uncond]; LoRA only on the student samples
+        eps_all = u.forward(self.noisy3[:nb * B], self.start_t3[:nb * B],
+                            self.in_ctx3 if nb == 3 else self.in_ctx3[:2 * B * 77],
+                            lora=True, save=True, lora_batch=B, added_cond=added(0, nb * B))
+        kv = u.last_ctx_kv
+        eps_s, eps_c = eps_all[:B], eps_all[B:2 * B]
+        eps_u = eps_all[2 * B:] if nb == 3 else eps_c
         # the target network is the student (same LoRA factors) on the same prompt embeddings
         # (T15:1192-1198 vs 1263-1268): its cross-attention k / v ARE the student rows of the pass above
         if kv is not None:

@@ -46,17 +46,14 @@ class UNetB200:
         # every resnet's time_emb_proj reads the same silu(temb): one grouped GEMM per pass
         # (1 base K entry + one N-ranged LoRA entry per layer must fit the K program)
         self._temb_names = [n for n, *_ in tab if n.endswith(".time_emb_proj")]
-        if not 2 <= len(self._temb_names) <= 23:
-            self._temb_names = []
+        if len(self._temb_names) > 23:
+            raise ValueError(f"{len(self._temb_names)} time_emb_proj layers: the grouped time-embedding GEMM "
+                             f"holds at most 23 (PCM_MAX_PROG - 1)")
         # every cross-attention k / v projection reads the same text context: a few grouped GEMMs per
         # pass (chunks of <= 11 transformer blocks of one width, _build_ctx_group) instead of one per block
-        import os as _os0
-        self._ctx_names = [n for n, _, ci, *_ in tab if n.endswith((".attn2.to_k", ".attn2.to_v"))]
+        self._ctx_names = [n for n, *_ in tab if n.endswith((".attn2.to_k", ".attn2.to_v"))]
         _co = {n: co for n, _, _, co, _ in tab}
         self._ctx_names.sort(key=lambda n: _co[n])        # stable: blocks of one width become neighbours
-        if (_os0.environ.get("PCM_CTX_GROUP", "1") == "0" or len(self._ctx_names) < 4 or
-                len({ci for n, _, ci, *_ in tab if n in set(self._ctx_names)}) != 1):
-            self._ctx_names = []
         master, entries, opnd_total = [], [], 0
         moff = 0
         no_dgrad = ("attn2.to_k", "attn2.to_v", "time_emb_proj")
@@ -157,9 +154,7 @@ class UNetB200:
         self._lb = (1, 1)
         # LoRA weight-gradient GEMMs are off the dgrad critical path (they only feed the optimiser):
         # they run on a side stream and fill SMs the main backward chain leaves idle
-        import os as _os
-        self.use_wstream = (torch.device(device).type == "cuda" and need_backward and lora and
-                            _os.environ.get("PCM_WGRAD_STREAM", "1") != "0")
+        self.use_wstream = torch.device(device).type == "cuda" and need_backward and lora
         self.wstream = torch.cuda.Stream(device=device) if self.use_wstream else None
         self._keep = []
 
@@ -169,7 +164,7 @@ class UNetB200:
     def _group_of(self, name):
         """Names of the shared-input Linear group `name` belongs to (attn1 q/k/v, attn2 k/v, all
         time_emb_proj layers), or None."""
-        if name.endswith(".time_emb_proj") and self._temb_names:
+        if name.endswith(".time_emb_proj"):
             return self._temb_names
         for _, sufs in self._GROUPS:
             for suf in sufs:
@@ -179,8 +174,8 @@ class UNetB200:
 
     def _unit_of(self, name):
         """Layers whose LoRA operand copies are laid out kind-major next to each other: the shared-input
-        group of `name`, widened to ALL cross-attention k / v layers when they run as context chunks."""
-        if self._ctx_names and name.endswith((".attn2.to_k", ".attn2.to_v")):
+        group of `name`, widened to ALL cross-attention k / v layers (they run as context chunks)."""
+        if name.endswith((".attn2.to_k", ".attn2.to_v")):
             return self._ctx_names
         return self._group_of(name)
 
@@ -219,9 +214,6 @@ class UNetB200:
     def _build_temb_group(self):
         """Stacked operands of the time-embedding projections: W [sum C_i, temb], bias [sum C_i] and
         the kind-major LoRA copies A [g*r, temb], s*B [sum C_i, r]."""
-        self.temb_group = None
-        if not self._temb_names:
-            return
         Ls = [self.layers[n] for n in self._temb_names]
         G = types.SimpleNamespace(names=self._temb_names, layers=Ls, g=len(Ls), cin=Ls[0].cin)
         assert all(L.cin == G.cin and L.bias is not None for L in Ls)
@@ -277,7 +269,7 @@ class UNetB200:
             return
         names = self._ctx_names
         Ls = [self.layers[n] for n in names]
-        assert all(L.bias is None for L in Ls) and len(names) % 2 == 0
+        assert all(L.bias is None and L.cin == Ls[0].cin for L in Ls) and len(names) % 2 == 0
         CG = types.SimpleNamespace(names=names, cin=Ls[0].cin, nl=len(names), chunks=[], where={})
         CG.lora = all(L.lora is not None for L in Ls)
         if CG.lora:
@@ -346,12 +338,9 @@ class UNetB200:
         """Store every frozen GEMM weight K-blocked ([K/64][N][64], pcm_bsrc.kblocked): the operand tile of
         a K block becomes one contiguous run in HBM.  Matters for the small-M layers (8x8 / 16x16 levels,
         target pass), which stream their weights once per launch: a row-major tile is N separate
-        128-byte segments K*2 bytes apart.  PCM_KBLOCK=0 keeps the row-major layout."""
-        import os as _os
-        if _os.environ.get("PCM_KBLOCK", "1") == "0":
-            return
+        128-byte segments K*2 bytes apart."""
         members = set()
-        for G in list(self.groups.values()) + ([self.temb_group] if self.temb_group is not None else []):
+        for G in list(self.groups.values()) + [self.temb_group]:
             members.update(id(L) for L in G.layers)
             G.w_stack = ops.kblock(G.w_stack)
             if getattr(G, "w_t_cat", None) is not None:
@@ -604,15 +593,12 @@ class UNetB200:
         cout = self.layers[p + ".conv1"].cout
         flat = [x.view(B * HW, x.shape[-1]) for x in xs]
         h = self.gn(p + ".norm1", flat, B, HW, 1e-5, True, save)
-        if self._temb is not None:
-            G = self.temb_group
-            i = G.index[p + ".time_emb_proj"]
-            out_all, T_all = self._temb
-            tproj = out_all[:, G.offs[i]:G.offs[i + 1]]
-            if save is not None:
-                save.append(("linear", p + ".time_emb_proj", [st[:self._lrows(st.shape[0])]], T_all, i * self.r))
-        else:
-            tproj = self.linear(p + ".time_emb_proj", [st], lora, save=save)
+        G = self.temb_group
+        i = G.index[p + ".time_emb_proj"]
+        out_all, T_all = self._temb
+        tproj = out_all[:, G.offs[i]:G.offs[i + 1]]
+        if save is not None:
+            save.append(("linear", p + ".time_emb_proj", [st[:self._lrows(st.shape[0])]], T_all, i * self.r))
         h = self.conv3(p + ".conv1", [h.view(B, H, W, cin)], lora, rowvec=tproj, save=save)
         h = self.gn(p + ".norm2", [h.view(B * HW, cout)], B, HW, 1e-5, True, save)
         if cin != cout:
@@ -649,12 +635,9 @@ class UNetB200:
             h = self.linear(t + ".attn1.to_out.0", [a], lora, residual=h, save=save)
             n = self.ln(t + ".norm2", h, save)
             q = self.linear(t + ".attn2.to_q", [n], lora, save=save)
-            if self._ctxkv is not None:
-                k, v, Tkv = self._ctxkv[t]
-                if save is not None:
-                    save.append(("lgroup", t + ".attn2.to_k", ctx[:self._lrows(ctx.shape[0])], Tkv))
-            else:
-                k, v = self.linear_group(t + ".attn2.to_k", ctx, lora, save=save)
+            k, v, Tkv = self._ctxkv[t]
+            if save is not None:
+                save.append(("lgroup", t + ".attn2.to_k", ctx[:self._lrows(ctx.shape[0])], Tkv))
             a = self.attention(q, k, v, B, S, ctx.shape[0] // B, save, heads)
             h = self.linear(t + ".attn2.to_out.0", [a], lora, residual=h, save=save)
             n = self.ln(t + ".norm3", h, save)
@@ -705,7 +688,7 @@ class UNetB200:
             add_in = torch.cat([text_embeds.to(BF16), tid.view(B, -1)], dim=1).contiguous()  # [B, 2816] glue
             ah = self.linear("add_embedding.linear_1", [add_in], False, act=1)
             st = self.linear("add_embedding.linear_2", [ah], False, residual=temb, act=1)
-        self._temb = self.temb_all(st, lora) if self.temb_group is not None else None
+        self._temb = self.temb_all(st, lora)
         # cross-attention k / v of every block: given (ctx_kv: another pass of this step already projected
         # the same context with the same weights) or computed here in a few grouped GEMMs
         if ctx_kv is not None:
@@ -942,10 +925,6 @@ class UNetB200:
         if q.stride(0) == 3 * Cc:     # self-attention: q/k/v are column views of one [M, 3C] matrix
             pk = self._new(q.shape[0], 3 * Cc)
             dq, dk, dv = pk[:, :Cc], pk[:, Cc:2 * Cc], pk[:, 2 * Cc:]
-        elif k.stride(0) == 2 * Cc:   # cross-attention: k/v views of one [B*77, 2C] matrix
-            dq = self._new(q.shape[0], Cc)
-            pk = self._new(k.shape[0], 2 * Cc)
-            dk, dv = pk[:, :Cc], pk[:, Cc:]
         else:
             # cross-attention, k/v are column windows of a context chunk [B*77, sum 2C] (ctx_kv_all):
             # dk/dv go to the same window of a gradient matrix of that shape (the attention kernels

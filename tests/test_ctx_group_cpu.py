@@ -18,9 +18,6 @@ def test_context_chunks_equal_per_layer_projections(monkeypatch, cfg_name, lora_
     from pcm_b200 import config, ops
     from pcm_b200.unet import UNetB200
     cfg = getattr(config, cfg_name)
-    import os
-    if os.environ.get("PCM_CTX_GROUP", "1") == "0":
-        pytest.skip("context chunks switched off")
     net, sd = build_net(cfg)
     assert net.ctx_group is not None and len(net.ctx_group.chunks) >= 1
     r, s = net.r, net.scale

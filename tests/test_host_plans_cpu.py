@@ -197,8 +197,6 @@ def test_grouped_backward_plan(monkeypatch, tiny, lead, need_dx):
         net.linear_group(t + lead, x, True, save=tape)
         rec = tape[0]
     else:
-        if net.ctx_group is None:
-            pytest.skip("PCM_CTX_GROUP=0")
         kv = net.ctx_kv_all(x, True)            # T = this block's window of the stacked context projection
         rec = ("lgroup", t + lead, x, kv[t][2])
         assert rec[3].stride(0) == net.ctx_group.nl * net.r

@@ -93,10 +93,9 @@ def test_merged_pass_is_student_plus_frozen_teacher(monkeypatch):
     # (same launches on the same student rows; torch's CPU matmul blocking may differ in the last bit)
     assert ((g_merged - net.lora_grad).norm() / net.lora_grad.norm()).item() < 1e-5 and g_merged.abs().max() > 0
     # the target pass of the step takes the student rows of the merged pass's context projections
-    if net.ctx_group is not None:          # (PCM_CTX_GROUP=0: per-block launches, nothing to reuse)
-        sub = net.ctx_kv_rows(kv, S)
-        again = net.forward(x[:1], ts[:1], ctx2[:S], lora=True, ctx_kv=sub)
-        assert torch.equal(again, stu)
+    sub = net.ctx_kv_rows(kv, S)
+    again = net.forward(x[:1], ts[:1], ctx2[:S], lora=True, ctx_kv=sub)
+    assert torch.equal(again, stu)
 
 
 VARIANTS = {
@@ -109,7 +108,7 @@ VARIANTS = {
 }
 
 
-@pytest.mark.parametrize("merge,variant", [("1", "reference"), ("0", "reference"), ("1", "v_prediction_l2"),
+@pytest.mark.parametrize("merge,variant", [("1", "reference"), ("1", "v_prediction_l2"),
                                            ("1", "no_cfg_solver"), ("1", "two_substeps"), ("1", "two_phases"),
                                            ("1", "ema_target")])
 def test_step_host_sequence_matches_the_oracle_iteration(monkeypatch, merge, variant):
@@ -120,8 +119,7 @@ def test_step_host_sequence_matches_the_oracle_iteration(monkeypatch, merge, var
     from oracle import pcm_ref, unet_ref
     from pcm_b200 import config, ops
     from pcm_b200.step import PCMTrainStep
-    monkeypatch.setenv("PCM_MERGE_PASSES", merge)
-    kw = dict(VARIANTS[variant])
+    kw =dict(VARIANTS[variant])
     B, hw, multiphase = 2, 8, kw.pop("multiphase", 4)
     ocfg = unet_ref.TINY
     P = unet_ref.init_params(ocfg, 0, lora_b_std=0.02)
