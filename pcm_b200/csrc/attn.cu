@@ -9,6 +9,7 @@
 //
 // Layout: q [B, Sq, H*D] (row stride ldq), k / v [B, Skv, H*D] (ldk / ldv), o like q;
 // lse, delta [B, H, Sq] fp32 (lse in log2 units of the scaled scores).
+#include <stdio.h>
 #include <stdlib.h>
 #include "common.cuh"
 #include "host_common.h"
@@ -549,9 +550,64 @@ int attn_bwd_wg(const void* q, const void* k, const void* v, const void* dout, c
 }
 using namespace pcm;
 
+// Head sizes both directions run: a multiple of 8 whose 16-padded width has an attn.cu instance
+// (DISPATCH_DP).  The forward's wgmma kernel would also take d = 104 / 112, but the backward cannot.
+static bool attn_head_dim_supported(int D) {
+  if (D < 8 || D > 160 || D % 8 != 0) return false;
+  const int dp = (D + 15) / 16 * 16;
+  return dp != 112 && dp != 144;
+}
+
+struct AttnPtr {
+  const void* ptr;
+  const char* name;
+};
+struct AttnLd {
+  int64_t ld;
+  const char* name;
+};
+
+// Every attention kernel reads q / k / v / o / dout and writes out / dq / dk / dv in 16-byte chunks
+// (TMA boxes, cp.async, uint4 loads): the base pointers must be 16-byte aligned and the row strides
+// multiples of 8 elements.  Checked before any CUDA call, so a bad layout is an error, never a launch.
+template <int NP>
+static int check_attn_args(int B, int H, int Sq, int Skv, int D, const AttnPtr (&ptrs)[NP],
+                           const AttnLd (&lds)[4]) {
+  char msg[160];
+  const struct { int v; const char* name; } dims[4] = {{B, "B"}, {H, "H"}, {Sq, "Sq"}, {Skv, "Skv"}};
+  for (const auto& d : dims)
+    if (d.v < 1) {
+      snprintf(msg, sizeof(msg), "attention: %s = %d must be >= 1", d.name, d.v);
+      return set_error(msg);
+    }
+  if (!attn_head_dim_supported(D)) {
+    snprintf(msg, sizeof(msg),
+             "attention: head dim %d is not supported (multiples of 8 up to 96, and 120, 128, 152, 160)", D);
+    return set_error(msg);
+  }
+  for (const auto& p : ptrs)
+    if ((reinterpret_cast<uintptr_t>(p.ptr) & 15) != 0) {
+      snprintf(msg, sizeof(msg), "attention: %s is not 16-byte aligned", p.name);
+      return set_error(msg);
+    }
+  const long long hd = static_cast<long long>(H) * D;
+  for (const auto& l : lds) {
+    if (l.ld % 8 != 0) {
+      snprintf(msg, sizeof(msg), "attention: %s = %lld is not a multiple of 8", l.name,
+               static_cast<long long>(l.ld));
+      return set_error(msg);
+    }
+    if (l.ld < hd) {
+      snprintf(msg, sizeof(msg), "attention: %s = %lld is less than H*D = %lld", l.name,
+               static_cast<long long>(l.ld), hd);
+      return set_error(msg);
+    }
+  }
+  return 0;
+}
+
 #define DISPATCH_DP(D, CALL)                                                     \
   do {                                                                           \
-    if ((D) % 8 != 0) return set_error("attention: head dim must be a multiple of 8"); \
     const int dp_ = ((D) + 15) / 16 * 16;                                        \
     switch (dp_) {                                                               \
       case 16: return CALL<16>(p, st);                                           \
@@ -569,6 +625,9 @@ using namespace pcm;
 extern "C" int pcm_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse,
                             int B, int H, int Sq, int Skv, int D, int64_t ldq, int64_t ldk,
                             int64_t ldv, int64_t ldo, float scale, void* stream) {
+  const AttnPtr ptrs[] = {{q, "q"}, {k, "k"}, {v, "v"}, {out, "out"}};
+  const int bad = check_attn_args(B, H, Sq, Skv, D, ptrs, {{ldq, "ldq"}, {ldk, "ldk"}, {ldv, "ldv"}, {ldo, "ldo"}});
+  if (bad) return bad;
   AttnParams p{};
   p.q = reinterpret_cast<const bf16*>(q);
   p.k = reinterpret_cast<const bf16*>(k);
@@ -579,7 +638,7 @@ extern "C" int pcm_attn_fwd(const void* q, const void* k, const void* v, void* o
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
   p.scale = scale;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // wgmma / TMA kernel (d <= 128); returns 1 when the shape or layout is not covered
+  // wgmma / TMA kernel for d <= 128; returns 1 for wider heads, which run the mma.sync kernel below
   const int rc = attn_fwd_wg(q, k, v, out, lse, B, H, Sq, Skv, D, ldq, ldk, ldv, ldo, scale, st);
   if (rc <= 0) return rc;
   DISPATCH_DP(D, launch_fwd);
@@ -589,6 +648,10 @@ extern "C" int pcm_attn_bwd(const void* q, const void* k, const void* v, const v
                             const void* dout, const float* lse, float* delta, void* dq, void* dk,
                             void* dv, int B, int H, int Sq, int Skv, int D, int64_t ldq,
                             int64_t ldk, int64_t ldv, int64_t ldo, float scale, void* stream) {
+  const AttnPtr ptrs[] = {{q, "q"}, {k, "k"}, {v, "v"}, {o, "o"}, {dout, "dout"},
+                          {dq, "dq"}, {dk, "dk"}, {dv, "dv"}};
+  const int bad = check_attn_args(B, H, Sq, Skv, D, ptrs, {{ldq, "ldq"}, {ldk, "ldk"}, {ldv, "ldv"}, {ldo, "ldo"}});
+  if (bad) return bad;
   AttnParams p{};
   p.q = reinterpret_cast<const bf16*>(q);
   p.k = reinterpret_cast<const bf16*>(k);
@@ -604,8 +667,8 @@ extern "C" int pcm_attn_bwd(const void* q, const void* k, const void* v, const v
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
   p.scale = scale;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (D <= 64 && D % 8 == 0) {
-    // wgmma / TMA kernels (d <= 64) after delta = rowsum(dO o O); return 1 when the layout is not covered
+  if (D <= 64) {
+    // wgmma / TMA kernels (d <= 64) after delta = rowsum(dO o O); wider heads run launch_bwd below
     const long long total = static_cast<long long>(B) * Sq * H;
     CUDA_TRY(launch_pdl(attn_delta_kernel, dim3(static_cast<unsigned>((total + 127) / 128)), dim3(128), 0, st, p));
     const int rc = attn_bwd_wg(q, k, v, dout, lse, delta, dq, dk, dv, B, H, Sq, Skv, D, ldq, ldk, ldv, ldo, scale, st);

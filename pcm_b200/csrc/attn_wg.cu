@@ -393,9 +393,11 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_bwd_wg_kernel(const __grid
 }
 
 // 3-D map (head columns, sequence, batch) with 64 x 64 SWIZZLE_128B boxes; rows past S and columns
-// past H*D read as zero.  Returns 1 when the layout cannot be described (pointer / stride alignment).
+// past H*D read as zero.  pcm_attn_fwd / pcm_attn_bwd have already checked that the base is 16-byte
+// aligned and ld a multiple of 8, as TMA requires.
 int encode_seq_map(CUtensorMap* m, const void* base, int HD, int S, int B, long long ld) {
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld & 7) != 0) return 1;
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld & 7) != 0)
+    return set_error("attention: tensor map base not 16-byte aligned or row stride not a multiple of 8");
   cuuint64_t dims[3] = {static_cast<cuuint64_t>(HD), static_cast<cuuint64_t>(S), static_cast<cuuint64_t>(B)};
   cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * 2, static_cast<cuuint64_t>(ld) * 2 * S};
   cuuint32_t box[3] = {64, 64, 1}, estr[3] = {1, 1, 1};
@@ -404,7 +406,7 @@ int encode_seq_map(CUtensorMap* m, const void* base, int HD, int S, int B, long 
 
 }  // namespace
 
-// Returns 0 on launch, < 0 on error, 1 when the shape is not covered (the caller runs attn.cu's kernel).
+// Returns 0 on launch, < 0 on error, 1 for d > 128 (the caller runs attn.cu's kernel).
 int attn_fwd_wg(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H, int Sq,
                 int Skv, int D, long long ldq, long long ldk, long long ldv, long long ldo, float scale,
                 cudaStream_t stream) {
@@ -412,9 +414,9 @@ int attn_fwd_wg(const void* q, const void* k, const void* v, void* out, float* l
   static AttnWgParams p;
   memset(&p, 0, sizeof(p));
   int rc;
-  if ((rc = encode_seq_map(&p.q_map, q, H * D, Sq, B, ldq)) != 0) return rc > 0 ? 1 : rc;
-  if ((rc = encode_seq_map(&p.k_map, k, H * D, Skv, B, ldk)) != 0) return rc > 0 ? 1 : rc;
-  if ((rc = encode_seq_map(&p.v_map, v, H * D, Skv, B, ldv)) != 0) return rc > 0 ? 1 : rc;
+  if ((rc = encode_seq_map(&p.q_map, q, H * D, Sq, B, ldq)) != 0) return rc;
+  if ((rc = encode_seq_map(&p.k_map, k, H * D, Skv, B, ldk)) != 0) return rc;
+  if ((rc = encode_seq_map(&p.v_map, v, H * D, Skv, B, ldv)) != 0) return rc;
   p.out = reinterpret_cast<bf16*>(out);
   p.lse = lse;
   p.H = H; p.Sq = Sq; p.Skv = Skv; p.D = D; p.ldo = ldo;
@@ -444,7 +446,7 @@ int attn_fwd_wg(const void* q, const void* k, const void* v, void* out, float* l
 }
 
 // dK, dV and dQ from q, k, v, dO and the forward's lse plus delta = rowsum(dO o O) (already computed).
-// Returns 0 on launch, < 0 on error, 1 when the shape is not covered (d > 64 or a layout TMA cannot map).
+// Returns 0 on launch, < 0 on error, 1 for d > 64 (the caller runs attn.cu's kernels).
 int attn_bwd_wg(const void* q, const void* k, const void* v, const void* dout, const float* lse,
                 const float* delta, void* dq, void* dk, void* dv, int B, int H, int Sq, int Skv, int D,
                 long long ldq, long long ldk, long long ldv, long long ldo, float scale, cudaStream_t stream) {
@@ -452,10 +454,10 @@ int attn_bwd_wg(const void* q, const void* k, const void* v, const void* dout, c
   static AttnBwdParams pk, pq;
   memset(&pk, 0, sizeof(pk));
   int rc;
-  if ((rc = encode_seq_map(&pk.fix0_map, k, H * D, Skv, B, ldk)) != 0) return rc > 0 ? 1 : rc;
-  if ((rc = encode_seq_map(&pk.fix1_map, v, H * D, Skv, B, ldv)) != 0) return rc > 0 ? 1 : rc;
-  if ((rc = encode_seq_map(&pk.str0_map, q, H * D, Sq, B, ldq)) != 0) return rc > 0 ? 1 : rc;
-  if ((rc = encode_seq_map(&pk.str1_map, dout, H * D, Sq, B, ldo)) != 0) return rc > 0 ? 1 : rc;
+  if ((rc = encode_seq_map(&pk.fix0_map, k, H * D, Skv, B, ldk)) != 0) return rc;
+  if ((rc = encode_seq_map(&pk.fix1_map, v, H * D, Skv, B, ldv)) != 0) return rc;
+  if ((rc = encode_seq_map(&pk.str0_map, q, H * D, Sq, B, ldq)) != 0) return rc;
+  if ((rc = encode_seq_map(&pk.str1_map, dout, H * D, Sq, B, ldo)) != 0) return rc;
   pk.lse = lse; pk.delta = delta;
   pk.H = H; pk.Sq = Sq; pk.Skv = Skv; pk.D = D;
   pk.c = scale * 1.4426950408889634f;
