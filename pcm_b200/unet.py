@@ -13,6 +13,9 @@ Parameters use diffusers state-dict names; LoRA factors live in ONE flat fp32 bu
 (`lora_master`), their gradients in `lora_grad`.
 """
 import types
+from collections import namedtuple
+from dataclasses import dataclass
+from typing import Optional
 
 import torch
 
@@ -23,6 +26,61 @@ BF16 = torch.bfloat16
 TAPS3 = ops.TAPS3
 # stride-2 3x3 pad-1: kernel index -> (input parity, shift in the parity plane)
 _S2 = ((1, -1), (0, 0), (1, 0))
+# per input parity p: the kernel indices that read parity plane p, with their shifts in that plane
+_S2_PLANE = [[(k, sh) for k, (par, sh) in enumerate(_S2) if par == p] for p in range(2)]
+
+
+# tape records: what the backward of one op needs (views of the LoRA samples' rows only).  `op` names the
+# op kind; T is the layer's LoRA down-projection x A^T (None: no adapter).
+LinearRec = namedtuple("LinearRec", "op name xs T")
+TembRec = namedtuple("TembRec", "op name xs T t_c0")     # time_emb_proj: its block of T starts at column t_c0
+GroupRec = namedtuple("GroupRec", "op lead x T")         # lead: key of UNetB200.groups
+ConvRec = namedtuple("ConvRec", "op name xs T stride")
+GNRec = namedtuple("GNRec", "op name xs stats eps silu B HW")
+LNRec = namedtuple("LNRec", "op name x stats")
+AttnRec = namedtuple("AttnRec", "op q k v out lse B Sq Skv heads")
+GegluRec = namedtuple("GegluRec", "op u")
+# one BasicTransformerBlock
+TBlockRec = namedtuple("TBlockRec", "norm1 attn1_qkv attn1 attn1_out norm2 attn2_q attn2_kv attn2 attn2_out "
+                                    "norm3 ff_in geglu ff_out")
+
+
+def _last(records):
+    """The record a primitive just appended to `records` (None when the pass keeps no tape)."""
+    return records[-1] if records is not None else None
+
+
+class _Block:
+    takes_skip = False      # the input was [hidden state, skip]: an up-path resnet
+    pushes_skip = False     # the output went onto the skip list: end of a down-path group, downsampler
+
+
+@dataclass
+class ResnetRec(_Block):
+    name: str
+    norm1: GNRec
+    temb: TembRec
+    conv1: ConvRec
+    norm2: GNRec
+    shortcut: Optional[LinearRec]
+    conv2: ConvRec
+    takes_skip: bool
+
+
+@dataclass
+class TransformerRec(_Block):
+    name: str
+    norm: GNRec
+    proj_in: LinearRec
+    blocks: list            # TBlockRec per transformer block
+    proj_out: LinearRec
+
+
+@dataclass
+class ResampleRec(_Block):
+    name: str
+    conv: ConvRec           # stride 2 (down), or after the nearest-2x upsample (up)
+    up: bool
 
 
 class _Lora:
@@ -179,6 +237,15 @@ class UNetB200:
             return self._ctx_names
         return self._group_of(name)
 
+    def _stacked(self, layers, kind, rows, cols):
+        """The `kind` ("a_fwd", "sb_fwd", "sb_t") operand copies of `layers`, laid out kind-major next to
+        each other in lora_opnd, as ONE [rows, cols] view."""
+        o = getattr(layers[0].lora, "o_" + kind)
+        v = self.lora_opnd[o:o + rows * cols].view(rows, cols)
+        last = getattr(layers[-1].lora, kind)
+        assert last.data_ptr() == v.view(-1)[-last.numel():].data_ptr()
+        return v
+
     def _build_groups(self, need_backward):
         """Stack the frozen weights (and view the kind-major LoRA operand copies) of every shared-input
         group so that q/k/v (resp. cross-attention k/v) run as ONE GEMM with N = g*C."""
@@ -201,14 +268,9 @@ class UNetB200:
                 G.lora = all(L.lora is not None for L in Ls)
                 if G.lora:
                     r, g = self.r, G.g
-                    lo0 = Ls[0].lora
-                    op = self.lora_opnd
-                    G.a_stack = op[lo0.o_a_fwd:lo0.o_a_fwd + g * r * G.cin].view(g * r, G.cin)
-                    G.sb_stack = op[lo0.o_sb_fwd:lo0.o_sb_fwd + g * G.cout * r].view(g * G.cout, r)
-                    G.sbt_stack = op[lo0.o_sb_t:lo0.o_sb_t + g * G.cout * r].view(g * r, G.cout)
-                    assert Ls[-1].lora.a_fwd.data_ptr() == G.a_stack[(g - 1) * r:].data_ptr()
-                    assert Ls[-1].lora.sb_fwd.data_ptr() == G.sb_stack[(g - 1) * G.cout:].data_ptr()
-                    assert Ls[-1].lora.sb_t.data_ptr() == G.sbt_stack[(g - 1) * r:].data_ptr()
+                    G.a_stack = self._stacked(Ls, "a_fwd", g * r, G.cin)
+                    G.sb_stack = self._stacked(Ls, "sb_fwd", g * G.cout, r)
+                    G.sbt_stack = self._stacked(Ls, "sb_t", g * r, G.cout)
                 self.groups[name] = G
 
     def _build_temb_group(self):
@@ -230,33 +292,41 @@ class UNetB200:
             L.w_fwd = G.w_stack[G.offs[i]:G.offs[i + 1]]
         G.lora = all(L.lora is not None for L in Ls)
         if G.lora:
-            r, g = self.r, G.g
-            lo0, op = Ls[0].lora, self.lora_opnd
-            G.a_stack = op[lo0.o_a_fwd:lo0.o_a_fwd + g * r * G.cin].view(g * r, G.cin)
-            G.sb_stack = op[lo0.o_sb_fwd:lo0.o_sb_fwd + G.n_total * r].view(G.n_total, r)
-            assert Ls[-1].lora.a_fwd.data_ptr() == G.a_stack[(g - 1) * r:].data_ptr()
-            assert Ls[-1].lora.sb_fwd.data_ptr() == G.sb_stack[G.offs[-2]:].data_ptr()
+            G.a_stack = self._stacked(Ls, "a_fwd", G.g * self.r, G.cin)
+            G.sb_stack = self._stacked(Ls, "sb_fwd", G.n_total, self.r)
         self.temb_group = G
+
+    def _lora_down(self, x, a_stack):
+        """T = x @ a_stack^T: the LoRA down-projections of several layers that read the same x."""
+        T = self._new(x.shape[0], a_stack.shape[0])
+        ops.gemm([ops.asrc_mat(x)], [ops.bsrc(a_stack)], [(0, 0, 0, 0, x.shape[1] // 64, 0, 0)], lin=True,
+                 M=x.shape[0], N=a_stack.shape[0], out=T)
+        return T
+
+    def _stacked_gemm(self, x, w_stack, T, sb_stack, ranges, N, *, block_n, bias=None, dep_a_src=None):
+        """out[M, N] = [x | T] @ [w_stack ; sb_stack]^T (+ bias): the frozen weights of several layers stacked
+        along N, then one LoRA K entry per layer that reads T columns [t_c0, t_c0 + r) and only feeds that
+        layer's output columns [n_lo, n_hi); ranges = [(t_c0, n_lo, n_hi)] (unused when T is None)."""
+        srcs, bs = [ops.asrc_mat(x)], [ops.bsrc(w_stack)]
+        prog = [(0, 0, 0, 0, x.shape[1] // 64, 0, 0)]
+        if T is not None:
+            srcs.append(ops.asrc_mat(T))
+            bs.append(ops.bsrc(sb_stack))
+            prog += [(1, 1, 0, 0, 1, t_c0, 0, n_lo, n_hi) for t_c0, n_lo, n_hi in ranges]
+        out = self._new(x.shape[0], N)
+        ops.gemm(srcs, bs, prog, lin=True, M=x.shape[0], N=N, out=out, bias=bias, block_n=block_n,
+                 dep_a_src=dep_a_src)
+        return out
 
     def temb_all(self, st, lora):
         """All time_emb_proj layers of one pass: out[B, sum C_i] = [st | T] @ [W ; N-ranged s*B_i]^T + b.
         Returns (out, T): resnet i uses the column view out[:, offs[i]:offs[i+1]] as its row vector and
         column block i of T for its LoRA weight gradients."""
-        G = self.temb_group
-        B = st.shape[0]
-        Ml = self._lrows(B)
-        srcs, bs = [ops.asrc_mat(st)], [ops.bsrc(G.w_stack)]
-        prog = [(0, 0, 0, 0, G.cin // 64, 0, 0)]
-        T = None
-        if lora and G.lora:
-            r = self.r
-            T = self._new(Ml, G.g * r)
-            ops.gemm([ops.asrc_mat(st[:Ml])], [ops.bsrc(G.a_stack)], prog, lin=True, M=Ml, N=G.g * r, out=T)
-            srcs.append(ops.asrc_mat(T))
-            bs.append(ops.bsrc(G.sb_stack))
-            prog = prog + [(1, 1, 0, 0, 1, i * r, 0, G.offs[i], G.offs[i + 1]) for i in range(G.g)]
-        out = self._new(B, G.n_total)
-        ops.gemm(srcs, bs, prog, lin=True, M=B, N=G.n_total, out=out, bias=G.bias, block_n=G.bn)
+        G, r = self.temb_group, self.r
+        T = self._lora_down(st[:self._lrows(st.shape[0])], G.a_stack) if lora and G.lora else None
+        out = self._stacked_gemm(st, G.w_stack, T, getattr(G, "sb_stack", None),
+                                 [(i * r, G.offs[i], G.offs[i + 1]) for i in range(G.g)], G.n_total,
+                                 block_n=G.bn, bias=G.bias)
         return out, T
 
     def _build_ctx_group(self):
@@ -273,9 +343,7 @@ class UNetB200:
         CG = types.SimpleNamespace(names=names, cin=Ls[0].cin, nl=len(names), chunks=[], where={})
         CG.lora = all(L.lora is not None for L in Ls)
         if CG.lora:
-            lo0, op = Ls[0].lora, self.lora_opnd
-            CG.a_stack = op[lo0.o_a_fwd:lo0.o_a_fwd + CG.nl * self.r * CG.cin].view(CG.nl * self.r, CG.cin)
-            assert Ls[-1].lora.a_fwd.data_ptr() == CG.a_stack[(CG.nl - 1) * self.r:].data_ptr()
+            CG.a_stack = self._stacked(Ls, "a_fwd", CG.nl * self.r, CG.cin)
         cur = None
         for b in range(len(names) // 2):
             lead = names[2 * b]
@@ -292,34 +360,18 @@ class UNetB200:
             ch.bn = 160 if ch.cout % 160 == 0 else 64
             ch.w_stack = torch.cat([G.w_stack for G in ch.blocks], 0).contiguous()
             if CG.lora:
-                lo = self.layers[names[ch.first]].lora
-                ch.sb_stack = self.lora_opnd[lo.o_sb_fwd:lo.o_sb_fwd + ch.n_total * self.r].view(ch.n_total, self.r)
-                last = ch.blocks[-1].layers[-1].lora
-                assert last.sb_fwd.data_ptr() == ch.sb_stack[ch.n_total - ch.cout:].data_ptr()
+                ch.sb_stack = self._stacked([L for G in ch.blocks for L in G.layers], "sb_fwd", ch.n_total, self.r)
         self.ctx_group = CG
 
     def ctx_kv_all(self, ctx, lora):
         """{transformer block: (k, v, T)} for one pass: k / v are column views [M, C] of the chunk outputs,
         T the block's two columns blocks [Ml, 2r] of the stacked LoRA down-projection (None without LoRA)."""
         CG, r = self.ctx_group, self.r
-        M = ctx.shape[0]
-        Ml = self._lrows(M)
-        base = [(0, 0, 0, 0, CG.cin // 64, 0, 0)]
-        T = None
-        if lora and CG.lora:
-            T = self._new(Ml, CG.nl * r)
-            ops.gemm([ops.asrc_mat(ctx[:Ml])], [ops.bsrc(CG.a_stack)], base, lin=True, M=Ml, N=CG.nl * r, out=T)
-        outs = []
-        for ch in CG.chunks:
-            srcs, bs, prog = [ops.asrc_mat(ctx)], [ops.bsrc(ch.w_stack)], list(base)
-            if T is not None:
-                srcs.append(ops.asrc_mat(T))
-                bs.append(ops.bsrc(ch.sb_stack))
-                prog += [(1, 1, 0, 0, 1, (ch.first + i) * r, 0, i * ch.cout, (i + 1) * ch.cout)
-                         for i in range(2 * len(ch.blocks))]
-            out = self._new(M, ch.n_total)
-            ops.gemm(srcs, bs, prog, lin=True, M=M, N=ch.n_total, out=out, block_n=ch.bn)
-            outs.append(out)
+        T = self._lora_down(ctx[:self._lrows(ctx.shape[0])], CG.a_stack) if lora and CG.lora else None
+        outs = [self._stacked_gemm(ctx, ch.w_stack, T, getattr(ch, "sb_stack", None),
+                                   [((ch.first + i) * r, i * ch.cout, (i + 1) * ch.cout)
+                                    for i in range(2 * len(ch.blocks))], ch.n_total, block_n=ch.bn)
+                for ch in CG.chunks]
         kv = {}
         for t, (c, j) in CG.where.items():
             ch, out = CG.chunks[c], outs[c]
@@ -471,7 +523,8 @@ class UNetB200:
         return srcs, prog
 
     def conv3(self, name, xs, lora, stride=1, rowvec=None, residual=None, out_fp32=False, save=None):
-        """3x3 pad-1 convolution (+LoRA) over NHWC sources xs (channel concat), fused epilogue."""
+        """3x3 pad-1 convolution (+LoRA) over NHWC sources xs (channel concat), fused epilogue; appends its
+        ConvRec to the list `save`."""
         L = self.layers[name]
         B, H, W, _ = xs[0].shape
         Ho, Wo = H // stride, W // stride
@@ -480,10 +533,10 @@ class UNetB200:
         bs = [ops.bsrc(L.w_fwd)]
         T = None
         lbn = self._lrows(B)   # samples that carry the LoRA adapter (the leading ones of the batch)
+        xl = xs if lbn == B else [x[:lbn] for x in xs]
         if lora and L.lora is not None:
             # T = A(x) only for the LoRA samples; the other samples see T rows that TMA zero-fills
             T = self._new(lbn, Ho, Wo, self.r)
-            xl = xs if lbn == B else [x[:lbn] for x in xs]
             srcs_l, prog_l = (srcs, prog) if lbn == B else self._conv_prog(xl, 3, stride, L.cin)
             ops.gemm(srcs_l, [ops.bsrc(L.lora.a_fwd)], prog_l, lin=False, M=lbn * Ho * Wo, N=self.r,
                      geo=(Wo, Ho), out=T.view(lbn * Ho * Wo, self.r))
@@ -495,11 +548,12 @@ class UNetB200:
                  rowvec=rowvec, residual=None if residual is None else residual.reshape(M, N),
                  round_bf16=out_fp32, dep_a_src=None if T is None else len(srcs) - 1)
         if save is not None:
-            save.append(("conv3", name, xs if lbn == B else [x[:lbn] for x in xs], T, stride))
+            save.append(ConvRec("conv3", name, xl, T, stride))
         return out
 
     def linear(self, name, xs, lora, residual=None, act=0, save=None):
-        """nn.Linear / 1x1 conv over [M, C] matrices xs (channel concat) (+LoRA), fused epilogue."""
+        """nn.Linear / 1x1 conv over [M, C] matrices xs (channel concat) (+LoRA), fused epilogue; appends its
+        LinearRec to the list `save`."""
         L = self.layers[name]
         M, N = xs[0].shape[0], L.cout
         srcs = [ops.asrc_mat(x) for x in xs]
@@ -510,9 +564,10 @@ class UNetB200:
         bs = [ops.bsrc(L.w_fwd)]
         T = None
         Ml = self._lrows(M)
+        xl = xs if Ml == M else [x[:Ml] for x in xs]
         if lora and L.lora is not None:
             T = self._new(Ml, self.r)
-            srcs_l = srcs if Ml == M else [ops.asrc_mat(x[:Ml]) for x in xs]
+            srcs_l = srcs if Ml == M else [ops.asrc_mat(x) for x in xl]
             ops.gemm(srcs_l, [ops.bsrc(L.lora.a_fwd)], prog, lin=True, M=Ml, N=self.r, out=T)
             prog = prog + [(len(srcs), 1, 0, 0, 1, 0, 0)]
             srcs = srcs + [ops.asrc_mat(T)]   # Ml rows: tiles past them read zeros (TMA bounds)
@@ -521,32 +576,23 @@ class UNetB200:
         ops.gemm(srcs, bs, prog, lin=True, M=M, N=N, out=out, bias=L.bias, residual=residual, act=act,
                  dep_a_src=None if T is None else len(srcs) - 1)
         if save is not None:
-            save.append(("linear", name, xs if Ml == M else [x[:Ml] for x in xs], T))
+            save.append(LinearRec("linear", name, xl, T))
         return out
 
     def linear_group(self, lead, x, lora, save=None):
         """The g Linear layers of a shared-input group (attn1 q/k/v, attn2 k/v) as ONE GEMM:
         out[M, g*C] = x @ [W_0; ...; W_g-1]^T, layer i's LoRA up-projection entering as a K block that
-        only feeds its own C output columns.  Returns the g column views of out."""
-        G = self.groups[lead]
-        g, Cc, r = G.g, G.cout, self.r
-        M = x.shape[0]
-        Ml = self._lrows(M)
-        srcs, bs = [ops.asrc_mat(x)], [ops.bsrc(G.w_stack)]
-        prog = [(0, 0, 0, 0, G.cin // 64, 0, 0)]
-        T = None
-        bn = 160 if Cc % 160 == 0 else 64
-        if lora and G.lora:
-            T = self._new(Ml, g * r)
-            ops.gemm([ops.asrc_mat(x[:Ml])], [ops.bsrc(G.a_stack)], prog, lin=True, M=Ml, N=g * r, out=T)
-            srcs.append(ops.asrc_mat(T))
-            bs.append(ops.bsrc(G.sb_stack))
-            prog = prog + [(1, 1, 0, 0, 1, i * r, 0, i * Cc, (i + 1) * Cc) for i in range(g)]
-        out = self._new(M, g * Cc)
-        ops.gemm(srcs, bs, prog, lin=True, M=M, N=g * Cc, out=out, block_n=bn,
-                 dep_a_src=None if T is None else 1)
+        only feeds its own C output columns.  Returns the g column views of out; appends its GroupRec to
+        the list `save`."""
+        G, r = self.groups[lead], self.r
+        g, Cc = G.g, G.cout
+        xl = x[:self._lrows(x.shape[0])]
+        T = self._lora_down(xl, G.a_stack) if lora and G.lora else None
+        out = self._stacked_gemm(x, G.w_stack, T, getattr(G, "sb_stack", None),
+                                 [(i * r, i * Cc, (i + 1) * Cc) for i in range(g)], g * Cc,
+                                 block_n=160 if Cc % 160 == 0 else 64, dep_a_src=None if T is None else 1)
         if save is not None:
-            save.append(("lgroup", lead, x[:Ml], T))
+            save.append(GroupRec("lgroup", lead, xl, T))
         return [out[:, i * Cc:(i + 1) * Cc] for i in range(g)]
 
     def gn(self, name, xs, B, HW, eps, silu, save=None):
@@ -558,7 +604,7 @@ class UNetB200:
                           B, HW, self.cfg.norm_num_groups)
         if save is not None:
             lb = self._lrows(B)
-            save.append(("gn", name, xs if lb == B else [x[:lb * HW] for x in xs], stats[:lb], eps, silu, lb, HW))
+            save.append(GNRec("gn", name, xs if lb == B else [x[:lb * HW] for x in xs], stats[:lb], eps, silu, lb, HW))
         return out
 
     def ln(self, name, x, save=None):
@@ -568,44 +614,49 @@ class UNetB200:
         ops.layernorm_fwd(x, L.gamma, L.beta, out, stats)
         if save is not None:
             Ml = self._lrows(x.shape[0])
-            save.append(("ln", name, x[:Ml], stats[:Ml]))
+            save.append(LNRec("ln", name, x[:Ml], stats[:Ml]))
         return out
 
-    def attention(self, q, k, v, B, Sq, Skv, save=None, heads=None):
-        Hh = heads or self.cfg.num_heads
-        D = q.shape[1] // Hh
+    def attention(self, q, k, v, B, Sq, Skv, heads, save=None):
+        D = q.shape[1] // heads
         out = self._new(q.shape[0], q.shape[1])
-        lse = self._new(B, Hh, Sq, dtype=torch.float32)
-        ops.attn_fwd(q, k, v, out, lse, B, Hh, Sq, Skv, D, D ** -0.5)
+        lse = self._new(B, heads, Sq, dtype=torch.float32)
+        ops.attn_fwd(q, k, v, out, lse, B, heads, Sq, Skv, D, D ** -0.5)
         if save is not None:
             lb = self._lrows(B)
-            save.append(("attn", q[:lb * Sq], k[:lb * Skv], v[:lb * Skv], out[:lb * Sq], lse[:lb], lb, Sq, Skv, Hh))
+            save.append(AttnRec("attn", q[:lb * Sq], k[:lb * Skv], v[:lb * Skv], out[:lb * Sq], lse[:lb], lb, Sq, Skv,
+                                heads))
         return out
 
     # ------------------------------------------------------------------------------------
-    # blocks (forward)
+    # blocks (forward): each returns (out, block record)
     # ------------------------------------------------------------------------------------
     def resnet(self, p, xs, st, lora, save):
-        """xs: list of NHWC sources (skip concat = 2 sources).  Returns [B,H,W,Cout]."""
+        """xs: list of NHWC sources (skip concat = 2 sources).  Returns ([B,H,W,Cout], ResnetRec)."""
         B, H, W, _ = xs[0].shape
         HW = H * W
         cin = sum(x.shape[-1] for x in xs)
         cout = self.layers[p + ".conv1"].cout
         flat = [x.view(B * HW, x.shape[-1]) for x in xs]
-        h = self.gn(p + ".norm1", flat, B, HW, 1e-5, True, save)
+        s = [] if save else None        # this block's op records
+        h = self.gn(p + ".norm1", flat, B, HW, 1e-5, True, s)
+        norm1 = _last(s)
         G = self.temb_group
         i = G.index[p + ".time_emb_proj"]
         out_all, T_all = self._temb
-        tproj = out_all[:, G.offs[i]:G.offs[i + 1]]
-        if save is not None:
-            save.append(("linear", p + ".time_emb_proj", [st[:self._lrows(st.shape[0])]], T_all, i * self.r))
-        h = self.conv3(p + ".conv1", [h.view(B, H, W, cin)], lora, rowvec=tproj, save=save)
-        h = self.gn(p + ".norm2", [h.view(B * HW, cout)], B, HW, 1e-5, True, save)
+        # the grouped launch of temb_all computed this layer: its record only names the column block
+        temb = TembRec("linear", p + ".time_emb_proj", [st[:self._lrows(st.shape[0])]], T_all, i * self.r)
+        h = self.conv3(p + ".conv1", [h.view(B, H, W, cin)], lora, rowvec=out_all[:, G.offs[i]:G.offs[i + 1]],
+                       save=s)
+        conv1 = _last(s)
+        h = self.gn(p + ".norm2", [h.view(B * HW, cout)], B, HW, 1e-5, True, s)
+        norm2 = _last(s)
+        sc, shortcut = xs[0], None
         if cin != cout:
-            sc = self.linear(p + ".conv_shortcut", flat, lora, save=save).view(B, H, W, cout)
-        else:
-            sc = xs[0]
-        return self.conv3(p + ".conv2", [h.view(B, H, W, cout)], lora, residual=sc, save=save)
+            sc = self.linear(p + ".conv_shortcut", flat, lora, save=s).view(B, H, W, cout)
+            shortcut = _last(s)
+        out = self.conv3(p + ".conv2", [h.view(B, H, W, cout)], lora, residual=sc, save=s)
+        return out, ResnetRec(p, norm1, temb, conv1, norm2, shortcut, _last(s), takes_skip=len(xs) == 2)
 
     def _level_of(self, name):
         """Resolution level of a block name (selects transformer depth and head count)."""
@@ -625,29 +676,48 @@ class UNetB200:
         level = self._level_of(p)
         heads = self.cfg.heads(level)
         xf = x.view(M, C)
-        g = self.gn(p + ".norm", [xf], B, S, 1e-6, False, save)
-        h = self.linear(p + ".proj_in", [g], lora, save=save)
+        s = [] if save else None        # this block's op records
+        g = self.gn(p + ".norm", [xf], B, S, 1e-6, False, s)
+        norm = _last(s)
+        h = self.linear(p + ".proj_in", [g], lora, save=s)
+        proj_in = _last(s)
+        blocks = []
         for d in range(self.cfg.depth(level)):
             t = p + f".transformer_blocks.{d}"
-            n = self.ln(t + ".norm1", h, save)
-            q, k, v = self.linear_group(t + ".attn1.to_q", n, lora, save=save)
-            a = self.attention(q, k, v, B, S, S, save, heads)
-            h = self.linear(t + ".attn1.to_out.0", [a], lora, residual=h, save=save)
-            n = self.ln(t + ".norm2", h, save)
-            q = self.linear(t + ".attn2.to_q", [n], lora, save=save)
+            b = [] if save else None    # the op records of one transformer block, in TBlockRec order
+            n = self.ln(t + ".norm1", h, b)
+            q, k, v = self.linear_group(t + ".attn1.to_q", n, lora, save=b)
+            a = self.attention(q, k, v, B, S, S, heads, b)
+            h = self.linear(t + ".attn1.to_out.0", [a], lora, residual=h, save=b)
+            n = self.ln(t + ".norm2", h, b)
+            q = self.linear(t + ".attn2.to_q", [n], lora, save=b)
             k, v, Tkv = self._ctxkv[t]
-            if save is not None:
-                save.append(("lgroup", t + ".attn2.to_k", ctx[:self._lrows(ctx.shape[0])], Tkv))
-            a = self.attention(q, k, v, B, S, ctx.shape[0] // B, save, heads)
-            h = self.linear(t + ".attn2.to_out.0", [a], lora, residual=h, save=save)
-            n = self.ln(t + ".norm3", h, save)
-            u = self.linear(t + ".ff.net.0.proj", [n], lora, save=save)
+            if save:    # k / v came from the context chunks of ctx_kv_all; Tkv is this block's window of T
+                b.append(GroupRec("lgroup", t + ".attn2.to_k", ctx[:self._lrows(ctx.shape[0])], Tkv))
+            a = self.attention(q, k, v, B, S, ctx.shape[0] // B, heads, b)
+            h = self.linear(t + ".attn2.to_out.0", [a], lora, residual=h, save=b)
+            n = self.ln(t + ".norm3", h, b)
+            u = self.linear(t + ".ff.net.0.proj", [n], lora, save=b)
             gg = self._new(M, u.shape[1] // 2)
             ops.geglu_fwd(u, gg)
-            if save is not None:
-                save.append(("geglu", u[:self._lrows(M)]))
-            h = self.linear(t + ".ff.net.2", [gg], lora, residual=h, save=save)
-        return self.linear(p + ".proj_out", [h], lora, residual=xf, save=save).view(B, H, W, C)
+            if save:
+                b.append(GegluRec("geglu", u[:self._lrows(M)]))
+            h = self.linear(t + ".ff.net.2", [gg], lora, residual=h, save=b)
+            blocks.append(TBlockRec._make(b) if save else None)
+        out = self.linear(p + ".proj_out", [h], lora, residual=xf, save=s)
+        return out.view(B, H, W, C), TransformerRec(p, norm, proj_in, blocks, _last(s))
+
+    def resample(self, name, x, lora, save, up):
+        """Downsampler (stride-2 convolution) or upsampler (nearest 2x, then the convolution)."""
+        s = [] if save else None
+        if not up:
+            out = self.conv3(name, [x], lora, stride=2, save=s)
+        else:
+            B, H, W, C = x.shape
+            xu = self._new(B, 2 * H, 2 * W, C)
+            ops.upsample2x_fwd(x, xu)
+            out = self.conv3(name, [xu], lora, save=s)
+        return out, ResampleRec(name, _last(s), up)
 
     def _lrows(self, n):
         """Rows / samples of an n-row (batch-major) tensor that belong to the LoRA samples."""
@@ -667,7 +737,6 @@ class UNetB200:
         holds views of the first b samples, so backward() is the student's backward."""
         cfg = self.cfg
         lora = lora and self.has_lora
-        tape = [] if save else None
         B, H, W, _ = sample.shape
         self._lb = (lora_batch if (lora and lora_batch) else B, B)
         c0 = cfg.block_out_channels[0]
@@ -700,84 +769,75 @@ class UNetB200:
         x = self._new(B, H, W, c0)
         Lci = self.layers["conv_in"]
         ops.conv3x3_c4(sample, Lci.w_c4, Lci.bias, x, sgn=1, round_in=True)
-        skips = [x]
+        tape, skips = [], [x]       # tape: the block records in forward order
+
+        def run(out_rec):
+            tape.append(out_rec[1])
+            return out_rec[0]
+
+        def push(x):                # the last block's output x becomes a skip input of the up path
+            tape[-1].pushes_skip = True
+            skips.append(x)
+
         nb = len(cfg.block_out_channels)
-        marks = []  # tape segment boundaries for the backward walk
         for i in range(nb):
             for j in range(cfg.layers_per_block):
-                x = self._block(tape, marks, "res", f"down_blocks.{i}.resnets.{j}", [x], st, lora)
+                x = run(self.resnet(f"down_blocks.{i}.resnets.{j}", [x], st, lora, save))
                 if cfg.down_attn[i]:
-                    x = self._block(tape, marks, "attn", f"down_blocks.{i}.attentions.{j}", x, ctx, lora)
-                skips.append(x)
+                    x = run(self.transformer(f"down_blocks.{i}.attentions.{j}", x, ctx, lora, save))
+                push(x)
             if i < nb - 1:
-                x = self._block(tape, marks, "down", f"down_blocks.{i}.downsamplers.0.conv", x, None, lora)
-                skips.append(x)
-        x = self._block(tape, marks, "res", "mid_block.resnets.0", [x], st, lora)
-        x = self._block(tape, marks, "attn", "mid_block.attentions.0", x, ctx, lora)
-        x = self._block(tape, marks, "res", "mid_block.resnets.1", [x], st, lora)
+                x = run(self.resample(f"down_blocks.{i}.downsamplers.0.conv", x, lora, save, up=False))
+                push(x)
+        x = run(self.resnet("mid_block.resnets.0", [x], st, lora, save))
+        x = run(self.transformer("mid_block.attentions.0", x, ctx, lora, save))
+        x = run(self.resnet("mid_block.resnets.1", [x], st, lora, save))
         for i in range(nb):
             for j in range(cfg.layers_per_block + 1):
-                x = self._block(tape, marks, "res", f"up_blocks.{i}.resnets.{j}", [x, skips.pop()], st, lora)
+                x = run(self.resnet(f"up_blocks.{i}.resnets.{j}", [x, skips.pop()], st, lora, save))
                 if cfg.up_attn[i]:
-                    x = self._block(tape, marks, "attn", f"up_blocks.{i}.attentions.{j}", x, ctx, lora)
+                    x = run(self.transformer(f"up_blocks.{i}.attentions.{j}", x, ctx, lora, save))
             if i < nb - 1:
-                x = self._block(tape, marks, "up", f"up_blocks.{i}.upsamplers.0.conv", x, None, lora)
+                x = run(self.resample(f"up_blocks.{i}.upsamplers.0.conv", x, lora, save, up=True))
         Bx, Hx, Wx, Cx = x.shape
-        g = self.gn("conv_norm_out", [x.view(Bx * Hx * Wx, Cx)], Bx, Hx * Wx, 1e-5, True, tape)
+        head = [] if save else None
+        g = self.gn("conv_norm_out", [x.view(Bx * Hx * Wx, Cx)], Bx, Hx * Wx, 1e-5, True, head)
         eps = self.conv3("conv_out", [g.view(Bx, Hx, Wx, Cx)], False, out_fp32=True)
         if save:
-            self.saved = (tape, marks, (self._lb[0], H, W))
+            self.saved = (tape, head[0], (self._lb[0], H, W))
         return eps
-
-    def _block(self, tape, marks, kind, name, x, aux, lora):
-        start = len(tape) if tape is not None else 0
-        if kind == "res":
-            out = self.resnet(name, x, aux, lora, tape)
-        elif kind == "attn":
-            out = self.transformer(name, x, aux, lora, tape)
-        elif kind == "down":
-            out = self.conv3(name, [x], lora, stride=2, save=tape)
-        else:  # up: nearest 2x then conv
-            B, H, W, C = x.shape
-            xu = self._new(B, 2 * H, 2 * W, C)
-            ops.upsample2x_fwd(x, xu)
-            out = self.conv3(name, [xu], lora, save=tape)
-        if tape is not None:
-            marks.append((kind, name, start, len(tape)))
-        return out
 
     # ------------------------------------------------------------------------------------
     # backward primitives
     # ------------------------------------------------------------------------------------
-    def _lora_wgrads(self, L, P_list, dy_mat, T_mat, dt_mat, taps_desc, lin, geo, M, q_c0=0):
-        """dB += s * dy^T T[:, q_c0:q_c0+r] ;  dA += dt^T x  (per source / tap group)."""
+    def _lora_wgrads(self, L, M, dy, T, dt, P_list, t_c0=0, dt_c0=0, lin=True, geo=(1, 1)):
+        """LoRA weight gradients of layer L (called inside _Side): dB += s * dy^T T[:, t_c0:t_c0+r] and
+        dA += dt[:, dt_c0:dt_c0+r]^T x for each (x, taps, tap offsets) of P_list.  dy, T, dt: A-operand
+        sources with M rows."""
         lo = L.lora
-        with UNetB200._Side(self, (dy_mat, T_mat, dt_mat, P_list)):
-            ops.wgrad(ops.asrc_mat(dy_mat), ops.asrc_mat(T_mat), lo.gB, lin=True, M=M, os_row=self.r, os_col=1,
-                      alpha=self.scale, q_c0=q_c0)
-            ktot = lo.gA.shape[1]
-            for (psrc, taps, offs) in P_list:
-                ops.wgrad(psrc, taps_desc(dt_mat), lo.gA, lin=lin, M=M, geo=geo, taps=taps, tap_off=offs,
-                          os_row=1, os_col=ktot)
+        ops.wgrad(dy, T, lo.gB, lin=True, M=M, os_row=self.r, os_col=1, alpha=self.scale, q_c0=t_c0)
+        for psrc, taps, offs in P_list:
+            ops.wgrad(psrc, dt, lo.gA, lin=lin, M=M, geo=geo, taps=taps, tap_off=offs, os_row=1,
+                      os_col=lo.gA.shape[1], q_c0=dt_c0)
 
-    def linear_bwd(self, rec, dy, need_dx=True, accumulate=None):
-        """rec = ("linear", name, xs, T[, q_c0]).  Returns dx [M, cin_total] (or None)."""
-        _, name, xs, T = rec[:4]
-        q_c0 = rec[4] if len(rec) > 4 else 0
-        L = self.layers[name]
+    def linear_bwd(self, rec, dy, need_dx=True, t_c0=0):
+        """rec: LinearRec (or TembRec, whose block of T starts at column t_c0).  Returns dx [M, cin_total]
+        (or None)."""
+        L = self.layers[rec.name]
         M = dy.shape[0]
-        srcs, bs = [ops.asrc_mat(dy)], None
+        srcs = [ops.asrc_mat(dy)]
         dt = None
-        if T is not None:
+        if rec.T is not None:
             dt = self._new(M, self.r)
             ops.gemm([ops.asrc_mat(dy)], [ops.bsrc(L.lora.sb_t)], [(0, 0, 0, 0, L.cout // 64, 0, 0)],
                      lin=True, M=M, N=self.r, out=dt)
             P_list, coff = [], 0
-            for x in xs:
+            for x in rec.xs:
                 P_list.append((ops.asrc_mat(x), ((0, 0),), (coff,)))
                 coff += x.shape[1]
-            self._keep.extend(xs)
-            self._lora_wgrads(L, P_list, dy, T, dt, ops.asrc_mat, True, (1, 1), M, q_c0=q_c0)
+            with UNetB200._Side(self, (dy, rec.T, dt, *rec.xs)):
+                self._lora_wgrads(L, M, ops.asrc_mat(dy), ops.asrc_mat(rec.T), ops.asrc_mat(dt), P_list,
+                                  t_c0=t_c0)
         if not need_dx:
             return None
         prog = [(0, 0, 0, 0, L.cout // 64, 0, 0)]
@@ -787,12 +847,11 @@ class UNetB200:
             bs.append(ops.bsrc(L.lora.a_t))
             prog.append((1, 1, 0, 0, 1, 0, 0))
         dx = self._new(M, L.cin)
-        ops.gemm(srcs, bs, prog, lin=True, M=M, N=L.cin, out=dx, residual=accumulate,
-                 dep_a_src=None if dt is None else 1)
+        ops.gemm(srcs, bs, prog, lin=True, M=M, N=L.cin, out=dx, dep_a_src=None if dt is None else 1)
         return dx
 
     def linear_group_bwd(self, rec, dpk, need_dx=True):
-        """rec = ("lgroup", lead, x, T); dpk [M, g*C] = the g output gradients side by side.
+        """rec: GroupRec ("lgroup", lead, x, T); dpk [M, g*C] = the g output gradients side by side.
         Returns dx [M, cin] (or None): ONE dgrad GEMM over K = g*C (+ the g LoRA blocks)."""
         _, lead, x, T = rec
         G = self.groups[lead]
@@ -806,10 +865,9 @@ class UNetB200:
                      block_n=64)
             with UNetB200._Side(self, (dpk, T, dT, x)):
                 for i, L in enumerate(G.layers):
-                    ops.wgrad(ops.asrc_mat(dpk[:, i * Cc:(i + 1) * Cc]), ops.asrc_mat(T), L.lora.gB, lin=True,
-                              M=M, os_row=r, os_col=1, alpha=self.scale, q_c0=i * r)
-                    ops.wgrad(ops.asrc_mat(x), ops.asrc_mat(dT), L.lora.gA, lin=True, M=M, os_row=1,
-                              os_col=G.cin, q_c0=i * r)
+                    self._lora_wgrads(L, M, ops.asrc_mat(dpk[:, i * Cc:(i + 1) * Cc]), ops.asrc_mat(T),
+                                      ops.asrc_mat(dT), [(ops.asrc_mat(x), ((0, 0),), (0,))],
+                                      t_c0=i * r, dt_c0=i * r)
         if not need_dx:
             return None
         srcs, bs = [ops.asrc_mat(dpk)], [ops.bsrc(G.w_t_cat)]
@@ -823,48 +881,37 @@ class UNetB200:
         ops.gemm(srcs, bs, prog, lin=True, M=M, N=G.cin, out=dx, dep_a_src=None if dT is None else 1)
         return dx
 
-    def conv3_bwd(self, rec, dy, need_dx=True, accumulate=None):
-        """rec = ("conv3", name, xs, T, stride); dy [B,Ho,Wo,N].  Returns dx [B,H,W,cin_total]."""
-        _, name, xs, T, stride = rec
-        L = self.layers[name]
+    def conv3_bwd(self, rec, dy, need_dx=True):
+        """rec: ConvRec; dy [B,Ho,Wo,N].  Returns dx [B,H,W,cin_total] (or None)."""
+        L = self.layers[rec.name]
         B, Ho, Wo, N = dy.shape
         M = B * Ho * Wo
         geo = (Wo, Ho)
         dy_m = dy.view(M, N)
         dt = None
-        if T is not None:
+        if rec.T is not None:
             dt = self._new(B, Ho, Wo, self.r)
             ops.gemm([ops.asrc_mat(dy_m)], [ops.bsrc(L.lora.sb_t)], [(0, 0, 0, 0, N // 64, 0, 0)],
                      lin=True, M=M, N=self.r, out=dt.view(M, self.r))
-            P_list = []
-            if stride == 1:
-                coff = 0
-                for x in xs:
+            if rec.stride == 1:
+                P_list, coff = [], 0
+                for x in rec.xs:
                     P_list.append((ops.asrc_nhwc(x), TAPS3, [t * L.cin + coff for t in range(9)]))
                     coff += x.shape[-1]
             else:
-                x = xs[0]
-                for p in range(2):
-                    for q in range(2):
-                        taps, offs = [], []
-                        for kh in range(3):
-                            for kw in range(3):
-                                if _S2[kh][0] == p and _S2[kw][0] == q:
-                                    taps.append((_S2[kw][1], _S2[kh][1]))
-                                    offs.append((kh * 3 + kw) * L.cin)
-                        P_list.append((ops.asrc_nhwc(x[:, p::2, q::2, :]), taps, offs))
-            lo = L.lora
-            with UNetB200._Side(self, (dy, T, dt, xs)):
-                ops.wgrad(ops.asrc_mat(dy_m), ops.asrc_mat(T.view(M, self.r)), lo.gB, lin=True, M=M,
-                          os_row=self.r, os_col=1, alpha=self.scale)
-                ktot = lo.gA.shape[1]
-                for (psrc, taps, offs) in P_list:
-                    ops.wgrad(psrc, ops.asrc_nhwc(dt), lo.gA, lin=False, M=M, geo=geo, taps=taps, tap_off=offs,
-                              os_row=1, os_col=ktot)
+                # parity plane (p, q) of x meets the kernel rows of _S2_PLANE[p] and columns of _S2_PLANE[q]
+                x = rec.xs[0]
+                P_list = [(ops.asrc_nhwc(x[:, p::2, q::2, :]),
+                           [(sw, sh) for kh, sh in _S2_PLANE[p] for kw, sw in _S2_PLANE[q]],
+                           [(kh * 3 + kw) * L.cin for kh, _ in _S2_PLANE[p] for kw, _ in _S2_PLANE[q]])
+                          for p in range(2) for q in range(2)]
+            with UNetB200._Side(self, (dy, rec.T, dt, rec.xs)):
+                self._lora_wgrads(L, M, ops.asrc_mat(dy_m), ops.asrc_mat(rec.T.view(M, self.r)),
+                                  ops.asrc_nhwc(dt), P_list, lin=False, geo=geo)
         if not need_dx:
             return None
         cin = L.cin
-        if stride == 1:
+        if rec.stride == 1:
             srcs, bs = [ops.asrc_nhwc(dy)], [ops.bsrc(L.w_t)]
             prog = [(0, 0, -dw, -dh, N // 64, 0, t * N) for t, (dw, dh) in enumerate(TAPS3)]
             if dt is not None:
@@ -873,53 +920,44 @@ class UNetB200:
                 prog += [(1, 1, -dw, -dh, 1, 0, t * self.r) for t, (dw, dh) in enumerate(TAPS3)]
             dx = self._new(B, Ho, Wo, cin)
             ops.gemm(srcs, bs, prog, lin=False, M=M, N=cin, geo=geo, out=dx.view(M, cin),
-                     residual=None if accumulate is None else accumulate.reshape(M, cin),
                      dep_a_src=None if dt is None else 1)
             return dx
-        # stride 2: one launch per parity plane of dx
+        # stride 2: one launch per parity plane of dx; x row 2i'+p receives dy row i'-sh through each
+        # kernel row (kh, sh) of _S2_PLANE[p] (and likewise for columns)
         H, W = 2 * Ho, 2 * Wo
         dx = self._new(B, H, W, cin)
         for p in range(2):
             for q in range(2):
-                # x row 2i'+p receives dy row i'+s through kernel row kh: p=0 -> (kh=1, s=0);
-                # p=1 -> (kh=0, s=+1), (kh=2, s=0)
-                khs = [(1, 0)] if p == 0 else [(0, 1), (2, 0)]
-                kws = [(1, 0)] if q == 0 else [(0, 1), (2, 0)]
-                srcs, bs, prog, lprog = [ops.asrc_nhwc(dy)], [ops.bsrc(L.w_t)], [], []
-                for kh, sh in khs:
-                    for kw, sw in kws:
-                        t = kh * 3 + kw
-                        prog.append((0, 0, sw, sh, N // 64, 0, t * N))
-                        lprog.append((1, 1, sw, sh, 1, 0, t * self.r))
+                taps = [(kh * 3 + kw, -sw, -sh) for kh, sh in _S2_PLANE[p] for kw, sw in _S2_PLANE[q]]
+                srcs, bs = [ops.asrc_nhwc(dy)], [ops.bsrc(L.w_t)]
+                prog = [(0, 0, dw, dh, N // 64, 0, t * N) for t, dw, dh in taps]
                 if dt is not None:
                     srcs.append(ops.asrc_nhwc(dt))
                     bs.append(ops.bsrc(L.lora.a_t))
-                    prog += lprog
+                    prog += [(1, 1, dw, dh, 1, 0, t * self.r) for t, dw, dh in taps]
                 plane = dx[:, p::2, q::2, :]
-                acc = None if accumulate is None else accumulate[:, p::2, q::2, :]
-                ops.gemm(srcs, bs, prog, lin=False, M=M, N=cin, geo=geo, out=plane, residual=acc,
+                ops.gemm(srcs, bs, prog, lin=False, M=M, N=cin, geo=geo, out=plane,
                          out_strides=(plane.stride(2), plane.stride(1), plane.stride(0)), epi=(Wo, Wo * Ho),
                          dep_a_src=1 if (dt is not None and p == 0 and q == 0) else None)
         return dx
 
     def gn_bwd(self, rec, dy, add=None, colsum=None):
-        _, name, xs, stats, eps, silu, B, HW = rec
-        L = self.layers[name]
+        L = self.layers[rec.name]
+        xs = rec.xs
         dx1 = torch.empty_like(xs[0])
         dx2 = torch.empty_like(xs[1]) if len(xs) > 1 else None
-        red = self._new(B, self.cfg.norm_num_groups, 2, dtype=torch.float32)
-        ops.groupnorm_bwd(dy, xs[0], xs[1] if len(xs) > 1 else None, L.gamma, L.beta, eps, silu, stats, red,
-                          add, dx1, dx2, B, HW, self.cfg.norm_num_groups, colsum=colsum)
+        red = self._new(rec.B, self.cfg.norm_num_groups, 2, dtype=torch.float32)
+        ops.groupnorm_bwd(dy, xs[0], xs[1] if len(xs) > 1 else None, L.gamma, L.beta, rec.eps, rec.silu,
+                          rec.stats, red, add, dx1, dx2, rec.B, rec.HW, self.cfg.norm_num_groups, colsum=colsum)
         return dx1, dx2
 
     def ln_bwd(self, rec, dy, add=None):
-        _, name, x, stats = rec
-        dx = torch.empty_like(x)
-        ops.layernorm_bwd(dy, x, self.layers[name].gamma, stats, add, dx)
+        dx = torch.empty_like(rec.x)
+        ops.layernorm_bwd(dy, rec.x, self.layers[rec.name].gamma, rec.stats, add, dx)
         return dx
 
     def attn_bwd(self, rec, dout):
-        _, q, k, v, out, lse, B, Sq, Skv, Hh = rec
+        q, k, v, Hh = rec.q, rec.k, rec.v, rec.heads
         D = q.shape[1] // Hh
         Cc = q.shape[1]
         if q.stride(0) == 3 * Cc:     # self-attention: q/k/v are column views of one [M, 3C] matrix
@@ -937,155 +975,108 @@ class UNetB200:
                 self._dkv_chunks[key] = self._new(k.shape[0], ld)
             pk = self._dkv_chunks[key][:, col0:col0 + 2 * Cc]
             dk, dv = pk[:, :Cc], pk[:, Cc:]
-        delta = torch.empty_like(lse)
-        ops.attn_bwd(q, k, v, out, dout, lse, delta, dq, dk, dv, B, Hh, Sq, Skv, D, D ** -0.5)
+        delta = torch.empty_like(rec.lse)
+        ops.attn_bwd(q, k, v, rec.out, dout, rec.lse, delta, dq, dk, dv, rec.B, Hh, rec.Sq, rec.Skv, D, D ** -0.5)
         return dq, pk
 
     # ------------------------------------------------------------------------------------
-    # block backward (records were appended in forward order)
+    # block backward
     # ------------------------------------------------------------------------------------
-    def resnet_bwd(self, recs, dout, need_dx=True):
-        """recs: [gn1, temb linear, conv1, gn2, (shortcut linear), conv2].  dout [B,H,W,Cout].
-        Returns (dx1, dx2) for the (possibly concatenated) input sources."""
-        has_sc = len(recs) == 6
-        gn1, tlin, conv1, gn2 = recs[0], recs[1], recs[2], recs[3]
-        conv2 = recs[-1]
+    def resnet_bwd(self, blk, dout, need_dx=True):
+        """dout [B,H,W,Cout].  Returns the gradients (NHWC) of the input and of the skip source (None
+        without a skip), or (None, None) without need_dx."""
         B, H, W, cout = dout.shape
         M = B * H * W
-        dh2 = self.conv3_bwd(conv2, dout)                              # grad wrt silu(gn2(h1))
+        dh2 = self.conv3_bwd(blk.conv2, dout)                          # grad wrt silu(gn2(h1))
         # grad wrt h1 [M, cout]; its per-image column sums (= d tproj[b, n], the time-embedding
         # branch) are accumulated by the same kernel
         cs32 = self._new(B, cout, dtype=torch.float32)
-        dh1, _ = self.gn_bwd(gn2, dh2.view(M, cout), colsum=cs32)
+        dh1, _ = self.gn_bwd(blk.norm2, dh2.view(M, cout), colsum=cs32)
         # the time-embedding branch ends in LoRA weight gradients only: all of it on the side stream
         with UNetB200._Side(self, (cs32,)):
             drow = self._new(B, cout)
             ops.cast_f32_bf16(cs32, drow)
             self._keep.append(drow)
-            self.linear_bwd(tlin, drow, need_dx=False)
-        dh = self.conv3_bwd(conv1, dh1.view(B, H, W, cout), need_dx=need_dx)
-        dsc = self.linear_bwd(recs[4], dout.view(M, cout), need_dx=need_dx) if has_sc else dout.view(M, cout)
+            self.linear_bwd(blk.temb, drow, need_dx=False, t_c0=blk.temb.t_c0)
+        dh = self.conv3_bwd(blk.conv1, dh1.view(B, H, W, cout), need_dx=need_dx)
+        dsc = dout.view(M, cout)
+        if blk.shortcut is not None:
+            dsc = self.linear_bwd(blk.shortcut, dsc, need_dx=need_dx)
         if not need_dx:
             return None, None
-        return self.gn_bwd(gn1, dh.view(M, -1), add=dsc)
+        dx1, dx2 = self.gn_bwd(blk.norm1, dh.view(M, -1), add=dsc)
+        return dx1.view(B, H, W, -1), None if dx2 is None else dx2.view(B, H, W, -1)
 
-    def transformer_bwd(self, recs, dout):
-        """recs order as appended by transformer(): gn, proj_in, depth x 13 block records, proj_out;
-        dout [B,H,W,C]; returns dx [B,H,W,C]."""
-        gn, pin, pout = recs[0], recs[1], recs[-1]
-        blocks = recs[2:-1]
-        assert len(blocks) % 13 == 0
+    def transformer_bwd(self, blk, dout):
+        """dout [B,H,W,C]; returns dx [B,H,W,C]."""
         B, H, W, C = dout.shape
         M = B * H * W
         do = dout.view(M, C)
-        dh = self.linear_bwd(pout, do)
-        for bi in reversed(range(len(blocks) // 13)):
-            (ln1, lqkv, at1, lo1, ln2, lq2, lkv2, at2, lo2, ln3, ff1, gegl, ff2) = blocks[13 * bi:13 * bi + 13]
+        dh = self.linear_bwd(blk.proj_out, do)
+        for b in reversed(blk.blocks):
             dh3 = dh
-            dgg = self.linear_bwd(ff2, dh3)
-            u = gegl[1]
-            du = torch.empty_like(u)
-            ops.geglu_bwd(dgg, u, du)
-            dn3 = self.linear_bwd(ff1, du)
-            dh2 = self.ln_bwd(ln3, dn3, add=dh3)
-            da2 = self.linear_bwd(lo2, dh2)
-            dq2, dkv2 = self.attn_bwd(at2, da2)
+            dgg = self.linear_bwd(b.ff_out, dh3)
+            du = torch.empty_like(b.geglu.u)
+            ops.geglu_bwd(dgg, b.geglu.u, du)
+            dn3 = self.linear_bwd(b.ff_in, du)
+            dh2 = self.ln_bwd(b.norm3, dn3, add=dh3)
+            da2 = self.linear_bwd(b.attn2_out, dh2)
+            dq2, dkv2 = self.attn_bwd(b.attn2, da2)
             with UNetB200._Side(self, (dkv2,)):     # feeds weight gradients only: off the dgrad chain
-                self.linear_group_bwd(lkv2, dkv2, need_dx=False)
-            dn2 = self.linear_bwd(lq2, dq2)
-            dh1 = self.ln_bwd(ln2, dn2, add=dh2)
-            da1 = self.linear_bwd(lo1, dh1)
-            _, dqkv = self.attn_bwd(at1, da1)
-            dn1 = self.linear_group_bwd(lqkv, dqkv)
-            dh = self.ln_bwd(ln1, dn1, add=dh1)
-        dg = self.linear_bwd(pin, dh)
-        dx, _ = self.gn_bwd(gn, dg, add=do)
+                self.linear_group_bwd(b.attn2_kv, dkv2, need_dx=False)
+            dn2 = self.linear_bwd(b.attn2_q, dq2)
+            dh1 = self.ln_bwd(b.norm2, dn2, add=dh2)
+            da1 = self.linear_bwd(b.attn1_out, dh1)
+            _, dqkv = self.attn_bwd(b.attn1, da1)
+            dn1 = self.linear_group_bwd(b.attn1_qkv, dqkv)
+            dh = self.ln_bwd(b.norm1, dn1, add=dh1)
+        dg = self.linear_bwd(blk.proj_in, dh)
+        dx, _ = self.gn_bwd(blk.norm, dg, add=do)
         return dx.view(B, H, W, C)
+
+    def resample_bwd(self, blk, dout):
+        dx = self.conv3_bwd(blk.conv, dout)
+        if not blk.up:
+            return dx
+        B, H, W, C = dx.shape
+        d = self._new(B, H // 2, W // 2, C)
+        ops.upsample2x_bwd(dx, d)
+        return d
 
     def backward(self, d_eps, grad_ready=None):
         """d_eps: fp32 [B,H,W,4] gradient of the loss w.r.t. the student epsilon.
         Accumulates LoRA gradients into self.lora_grad (caller zeroes it between steps).
         grad_ready(offset): called (on the weight-gradient stream) after each block's backward with
         the flat-buffer offset from which every gradient element is final."""
-        tape, marks, (B, H, W) = self.saved
+        tape, head, (B, H, W) = self.saved
         self._dkv_chunks = {}
         boffs = self.block_grad_offsets() if grad_ready is not None else None
-        pending = []
-        cfg = self.cfg
-        c0 = cfg.block_out_channels[0]
         Lco = self.layers["conv_out"]
+        c0 = Lco.cin
         dg = self._new(B, H, W, c0)
         ops.conv3x3_c4(d_eps, Lco.w_c4_t, None, dg, sgn=-1, round_in=False)
-        d, _ = self.gn_bwd(tape[-1], dg.view(B * H * W, c0))
+        d, _ = self.gn_bwd(head, dg.view(B * H * W, c0))
         d = d.view(B, H, W, c0)
-        nb = len(cfg.block_out_channels)
-        mi = len(marks) - 1
-        dskips = []
-
-        def pop():
-            nonlocal mi
-            # the block popped previously has been fully enqueued by now: its gradients are final once
-            # the weight-gradient stream drains
-            if grad_ready is not None and pending:
-                off = boffs.get(pending.pop())
-                if off is not None:
-                    with UNetB200._Side(self, ()):
-                        grad_ready(off)
-            kind, name, s, e = marks[mi]
-            mi -= 1
-            pending.append(name)
-            return kind, tape[s:e]
-
-        # up path (reverse)
-        for i in reversed(range(nb)):
-            if i < nb - 1:
-                _, recs = pop()
-                dxu = self.conv3_bwd(recs[0], d)
-                Bu, Hu, Wu, Cu = dxu.shape
-                d = self._new(Bu, Hu // 2, Wu // 2, Cu)
-                ops.upsample2x_bwd(dxu, d)
-            for j in reversed(range(cfg.layers_per_block + 1)):
-                if cfg.up_attn[i]:
-                    _, recs = pop()
-                    d = self.transformer_bwd(recs, d)
-                _, recs = pop()
-                d1, d2 = self.resnet_bwd(recs, d)
-                Bc, Hc, Wc, _ = d.shape
-                dskips.append(d2.view(Bc, Hc, Wc, -1))
-                d = d1.view(Bc, Hc, Wc, -1)
-        # mid
-        for kind in ("res", "attn", "res"):
-            k_, recs = pop()
-            if k_ == "attn":
-                d = self.transformer_bwd(recs, d)
+        dskips = []     # gradients of the up path's skip inputs; the last one left (conv_in's output) is unused
+        done = None     # the block walked before the current one
+        for i in reversed(range(len(tape))):
+            blk = tape[i]
+            if blk.pushes_skip:
+                d = ops.add_bf16(d, dskips.pop(), torch.empty_like(d))
+            # the block walked before has been fully enqueued by now: its gradients are final once the
+            # weight-gradient stream drains
+            if grad_ready is not None and boffs.get(done) is not None:
+                with UNetB200._Side(self, ()):
+                    grad_ready(boffs[done])
+            if isinstance(blk, ResnetRec):
+                d, dskip = self.resnet_bwd(blk, d, need_dx=i > 0)
+                if blk.takes_skip:
+                    dskips.append(dskip)
+            elif isinstance(blk, TransformerRec):
+                d = self.transformer_bwd(blk, d)
             else:
-                Bc, Hc, Wc, _ = d.shape
-                d = self.resnet_bwd(recs, d)[0].view(Bc, Hc, Wc, -1)
-        # down path (reverse); dskips is ordered s0..s11 reversed consumption -> s_last first
-        def add_skip(dcur):
-            ds = dskips_by_idx.pop()
-            out = torch.empty_like(dcur)
-            ops.add_bf16(dcur, ds, out)
-            return out
-
-        # up-path backward visited resnets in reverse, so dskips = [ds_0, ds_1, ..., ds_11]
-        dskips_by_idx = dskips  # pop() from the end = highest skip index first
-        for i in reversed(range(nb)):
-            if i < nb - 1:
-                d = add_skip(d)
-                _, recs = pop()
-                d = self.conv3_bwd(recs[0], d)
-            for j in reversed(range(cfg.layers_per_block)):
-                d = add_skip(d)
-                if cfg.down_attn[i]:
-                    _, recs = pop()
-                    d = self.transformer_bwd(recs, d)
-                _, recs = pop()
-                first = (i == 0 and j == 0)
-                Bc, Hc, Wc, _ = d.shape
-                r = self.resnet_bwd(recs, d, need_dx=not first)
-                if not first:
-                    d = r[0].view(Bc, Hc, Wc, -1)
+                d = self.resample_bwd(blk, d)
+            done = blk.name
         if grad_ready is not None:
             with UNetB200._Side(self, ()):
                 grad_ready(0)
