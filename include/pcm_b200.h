@@ -128,6 +128,13 @@ int64_t pcm_groupnorm_ws_bytes(int B, int HW, int C, int G);
 int pcm_groupnorm_fwd(const void* x1, const void* x2, int C1, int C2, int B, int HW, int G,
                       const float* gamma, const float* beta, float eps, int silu, void* out,
                       float* stats, void* ws, int64_t ws_bytes, void* stream);
+/* pcm_groupnorm_fwd over B images, with the per-image block partition of a launch over part_B >= B
+ * images: the statistics of image b are merged from the same partials, in the same order, as in that
+ * launch, so the outputs are bitwise equal to its rows of images 0..B-1.  Used when the leading images
+ * of a batch are normalised again on their own (gradient checkpointing). */
+int pcm_groupnorm_fwd_part(const void* x1, const void* x2, int C1, int C2, int B, int part_B, int HW,
+                           int G, const float* gamma, const float* beta, float eps, int silu, void* out,
+                           float* stats, void* ws, int64_t ws_bytes, void* stream);
 int pcm_groupnorm_bwd(const void* dy, const void* x1, const void* x2, int C1, int C2, int B, int HW,
                       int G, const float* gamma, const float* beta, float eps, int silu,
                       const float* stats, float* red, const void* add, void* dx1, void* dx2,

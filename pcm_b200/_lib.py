@@ -86,6 +86,7 @@ EXPORTS = [
     "pcm_wgrad",
     "pcm_groupnorm_ws_bytes",
     "pcm_groupnorm_fwd",
+    "pcm_groupnorm_fwd_part",
     "pcm_groupnorm_bwd",
     "pcm_layernorm_fwd",
     "pcm_layernorm_bwd",
@@ -121,6 +122,7 @@ ARGTYPES = {
     "pcm_wgrad": [P, P],
     "pcm_groupnorm_ws_bytes": [I, I, I, I],
     "pcm_groupnorm_fwd": [P, P, I, I, I, I, I, P, P, F, I, P, P, P, L64, P],
+    "pcm_groupnorm_fwd_part": [P, P, I, I, I, I, I, I, P, P, F, I, P, P, P, L64, P],
     "pcm_groupnorm_bwd": [P, P, P, I, I, I, I, I, P, P, F, I, P, P, P, P, P, P, P, L64, P],
     "pcm_layernorm_fwd": [P, I, I, P, P, F, P, P, P],
     "pcm_layernorm_bwd": [P, P, I, I, P, P, P, P, P],

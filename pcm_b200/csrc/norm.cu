@@ -692,17 +692,27 @@ extern "C" int pcm_groupnorm_fwd(const void* x1_, const void* x2_, int C1, int C
                                  int G, const float* gamma, const float* beta, float eps, int silu,
                                  void* out_, float* stats, void* ws, int64_t ws_bytes,
                                  void* stream_) {
+  return pcm_groupnorm_fwd_part(x1_, x2_, C1, C2, B, B, HW, G, gamma, beta, eps, silu, out_, stats, ws,
+                                ws_bytes, stream_);
+}
+
+extern "C" int pcm_groupnorm_fwd_part(const void* x1_, const void* x2_, int C1, int C2, int B,
+                                      int part_B, int HW, int G, const float* gamma, const float* beta,
+                                      float eps, int silu, void* out_, float* stats, void* ws,
+                                      int64_t ws_bytes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const int C = C1 + C2;
   if (C % G != 0 || C1 % 8 != 0 || C2 % 8 != 0) return set_error("groupnorm: bad channel split");
   if (B > kGnMaxB) return set_error("groupnorm: batch too large for the counter workspace");
+  if (part_B < B) return set_error("groupnorm: part_B must be >= B");
   const bf16* x1 = reinterpret_cast<const bf16*>(x1_);
   const bf16* x2 = reinterpret_cast<const bf16*>(x2_);
   bf16* out = reinterpret_cast<bf16*>(out_);
   unsigned* counters = reinterpret_cast<unsigned*>(ws);
   float* part = reinterpret_cast<float*>(counters + 3 * kGnMaxB);
   int threads, ppb, nblk;
-  if (int rc = gn_launch_cfg(C, HW, B, &threads, &ppb, &nblk)) return rc;
+  // the per-image partition (pixels per block) is the one a launch over part_B images would use
+  if (int rc = gn_launch_cfg(C, HW, part_B, &threads, &ppb, &nblk)) return rc;
   if (ws == nullptr || static_cast<size_t>(ws_bytes) < gn_ws_need(B, nblk, C, G))
     return set_error("groupnorm: workspace too small (see pcm_groupnorm_ws_bytes)");
   CUDA_TRY(launch_pdl(gn_stats_kernel, dim3(nblk, B), dim3(threads), 0, stream, x1, x2, C1, C2,

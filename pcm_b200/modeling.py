@@ -44,7 +44,10 @@ class UNet2DConditionModel:
         return [self.net.lora_master] if self.use_lora and self.net.has_lora else []
 
     def enable_gradient_checkpointing(self):
-        """No recompute is needed: the bs 8 SD1.5 step fits an 80 GB H100 without it; accepted for API parity."""
+        """Calls with save_for_backward=True keep only each block's inputs; backward() runs every ResNet /
+        Transformer2D / resample block's forward again right before that block's backward (diffusers
+        checkpoints the same blocks).  Less memory, one more forward of compute, the same gradients."""
+        self.net.gradient_checkpointing = True
 
     def enable_xformers_memory_efficient_attention(self):
         """Attention always runs the library's flash kernels; accepted for API parity."""

@@ -56,7 +56,7 @@ LAUNCHES = {"count": 0}
 PROFILE = None  # list of (start_event, end_event, flops) when enabled
 PROFILE_EXTERNAL = False  # True: events become event-record NODES when captured in a CUDA graph
 DRY_RUN = None  # list: record (kind, info) instead of launching (shape analysis without a GPU)
-_KERNELS_PER_CALL = {"pcm_groupnorm_fwd": 2, "pcm_groupnorm_bwd": 2, "pcm_attn_bwd": 3, "pcm_adamw_clip": 2}
+_KERNELS_PER_CALL = {"pcm_groupnorm_fwd": 2, "pcm_groupnorm_fwd_part": 2, "pcm_groupnorm_bwd": 2, "pcm_attn_bwd": 3, "pcm_adamw_clip": 2}
 
 
 
@@ -280,6 +280,18 @@ def groupnorm_fwd(x1, x2, gamma, beta, eps, silu, out, stats, B, HW, G=32):
     ws, nws = gn_workspace(x1.device, B, HW, C1 + C2, G)
     _call("pcm_groupnorm_fwd", _p(x1), _p(x2), C1, C2, B, HW, G, _p(gamma), _p(beta), eps, int(silu),
           _p(out), _p(stats), _p(ws), nws)
+    return out
+
+
+def groupnorm_fwd_part(x1, x2, gamma, beta, eps, silu, out, stats, B, part_B, HW, G=32):
+    """groupnorm_fwd over B images, with the per-image block partition of a launch over part_B >= B
+    images: bitwise equal to rows 0..B-1 of that launch (a block rebuilt for the backward from the
+    leading samples of a merged batch)."""
+    C1 = x1.shape[-1]
+    C2 = x2.shape[-1] if x2 is not None else 0
+    ws, nws = gn_workspace(x1.device, B, HW, C1 + C2, G)
+    _call("pcm_groupnorm_fwd_part", _p(x1), _p(x2), C1, C2, B, part_B, HW, G, _p(gamma), _p(beta), eps,
+          int(silu), _p(out), _p(stats), _p(ws), nws)
     return out
 
 

@@ -36,14 +36,18 @@ class PCMTrainStep:
                  lr=5e-6, betas=(0.9, 0.999), adam_eps=1e-8, weight_decay=1e-2, max_grad_norm=1.0,
                  apply_cfg_solver=True, bf16_mode=True, alphas_cumprod=None, process_group=None,
                  keep_debug=False, prediction_type="epsilon", ema_decay=None, grad_buckets=4,
-                 teacher_substeps=1):
+                 teacher_substeps=1, gradient_checkpointing=False):
         """prediction_type: "epsilon" | "v_prediction" (predicted_origin, T15:268-280).
         ema_decay: None (reference behaviour: the target network IS the student, update_ema is never
         called, T15:1261-1268) or a rate in (0, 1): opt-in EMA target, updated after every optimiser
         step as update_ema does (T15:344-355).
         teacher_substeps: 1 (reference behaviour: ONE DDIM step of the teacher over the 20-timestep
         interval, T15:1217-1258) or k > 1 dividing the interval: the teacher is evaluated k times along
-        it (opt-in multi-substep solve; each extra sub-step costs two more teacher forwards)."""
+        it (opt-in multi-substep solve; each extra sub-step costs two more teacher forwards).
+        gradient_checkpointing: the merged pass keeps only the student rows of each UNet block's inputs and
+        the backward runs every block's student forward again right before its backward (diffusers'
+        per-block torch.utils.checkpoint): less memory, one more student forward per step, the same
+        numbers bit for bit."""
         ratio = num_train_timesteps // num_ddim_timesteps
         if teacher_substeps < 1 or ratio % teacher_substeps != 0:
             raise ValueError(f"teacher_substeps must divide the DDIM interval ({ratio} train timesteps)")
@@ -54,7 +58,8 @@ class PCMTrainStep:
         self.cfg, self.dev = cfg, device
         self.B, self.H, self.W = batch, height, width
         self.per = height * width * 4
-        self.unet = UNetB200(cfg, state_dict, device, need_backward=True, lora=True)
+        self.unet = UNetB200(cfg, state_dict, device, need_backward=True, lora=True,
+                             gradient_checkpointing=gradient_checkpointing)
         self.multiphase, self.num_ddim, self.num_train = multiphase, num_ddim_timesteps, num_train_timesteps
         self.loss_type = 0 if loss_type == "huber" else 1
         self.huber_c = huber_c

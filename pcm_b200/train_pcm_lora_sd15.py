@@ -201,7 +201,8 @@ def main(args):
                       huber_c=args.huber_c, lr=args.learning_rate, betas=(args.adam_beta1, args.adam_beta2),
                       adam_eps=args.adam_epsilon, weight_decay=args.adam_weight_decay,
                       max_grad_norm=args.max_grad_norm, apply_cfg_solver=not args.not_apply_cfg_solver,
-                      process_group=pg, prediction_type=args.prediction_type, ema_decay=args.ema_decay)
+                      process_group=pg, prediction_type=args.prediction_type, ema_decay=args.ema_decay,
+                      gradient_checkpointing=args.gradient_checkpointing)
     del sd
     files = sorted(glob.glob(os.path.join(args.latent_cache, "*.pt"))) if args.latent_cache else []
     if not files and not args.synthetic:

@@ -13,6 +13,7 @@ Parameters use diffusers state-dict names; LoRA factors live in ONE flat fp32 bu
 (`lora_master`), their gradients in `lora_grad`.
 """
 import types
+import weakref
 from collections import namedtuple
 from dataclasses import dataclass
 from typing import Optional
@@ -83,6 +84,16 @@ class ResampleRec(_Block):
     up: bool
 
 
+@dataclass
+class CheckpointRec(_Block):
+    """A block of a gradient-checkpointed forward: what rebuilding its full record in backward() takes."""
+    kind: str               # "resnet" | "transformer" | "resample" (the UNetB200 method that runs it)
+    name: str
+    xs: list                # its inputs, student rows only, each an owned copy (an upsampler: before the 2x)
+    takes_skip: bool
+    up: bool = False
+
+
 class _Lora:
     __slots__ = ("a_off", "b_off", "a_fwd", "sb_fwd", "sb_t", "a_t", "gA", "gB", "opnd_off",
                  "o_a_fwd", "o_sb_fwd", "o_sb_t", "o_a_t")
@@ -94,8 +105,15 @@ class _Layer:
 
 
 class UNetB200:
-    def __init__(self, cfg: UNetConfig, state_dict, device, need_backward=True, lora=True):
+    gradient_checkpointing = False
+    _plan_b = None
+
+    def __init__(self, cfg: UNetConfig, state_dict, device, need_backward=True, lora=True,
+                 gradient_checkpointing=False):
+        """gradient_checkpointing: a forward with save=True keeps only the student rows of every block's
+        inputs; backward() runs each block's forward again right before its backward (see forward())."""
         self.cfg, self.dev = cfg, device
+        self.gradient_checkpointing = gradient_checkpointing
         self.r = cfg.lora_rank
         self.scale = cfg.lora_scale
         self.layers = {}
@@ -210,6 +228,9 @@ class UNetB200:
         self._ctxkv = self.last_ctx_kv = None
         self._dkv_chunks = {}
         self._lb = (1, 1)
+        # while backward() rebuilds a checkpointed block: the batch of the merged pass that first ran it,
+        # whose launch plans the rebuild keeps (_merged_tiling, gn)
+        self._plan_b = None
         # LoRA weight-gradient GEMMs are off the dgrad critical path (they only feed the optimiser):
         # they run on a side stream and fill SMs the main backward chain leaves idle
         self.use_wstream = torch.device(device).type == "cuda" and need_backward and lora
@@ -522,6 +543,16 @@ class UNetB200:
             coff += ci
         return srcs, prog
 
+    def _merged_tiling(self, M, N, prog):
+        """Tiling keywords of a block's main GEMM.  Empty (ops.gemm picks from M) except while backward()
+        rebuilds a checkpointed block: then the (block_n, ksplit) the merged pass picked for its larger M,
+        since pick_tiling splits K by M and the split decides how the fp32 sums round.  The LoRA
+        down-projections already ran on the student rows alone and need nothing."""
+        if self._plan_b is None:
+            return {}
+        bn, ks = ops.pick_tiling(M * self._plan_b // self._lb[1], N, sum(e[4] for e in prog))
+        return dict(block_n=bn, ksplit=ks)
+
     def conv3(self, name, xs, lora, stride=1, rowvec=None, residual=None, out_fp32=False, save=None):
         """3x3 pad-1 convolution (+LoRA) over NHWC sources xs (channel concat), fused epilogue; appends its
         ConvRec to the list `save`."""
@@ -546,7 +577,8 @@ class UNetB200:
         out = self._new(B, Ho, Wo, N, dtype=torch.float32 if out_fp32 else BF16)
         ops.gemm(srcs, bs, prog, lin=False, M=M, N=N, geo=(Wo, Ho), out=out.view(M, N), bias=L.bias,
                  rowvec=rowvec, residual=None if residual is None else residual.reshape(M, N),
-                 round_bf16=out_fp32, dep_a_src=None if T is None else len(srcs) - 1)
+                 round_bf16=out_fp32, dep_a_src=None if T is None else len(srcs) - 1,
+                 **self._merged_tiling(M, N, prog))
         if save is not None:
             save.append(ConvRec("conv3", name, xl, T, stride))
         return out
@@ -574,7 +606,7 @@ class UNetB200:
             bs.append(ops.bsrc(L.lora.sb_fwd))
         out = self._new(M, N)
         ops.gemm(srcs, bs, prog, lin=True, M=M, N=N, out=out, bias=L.bias, residual=residual, act=act,
-                 dep_a_src=None if T is None else len(srcs) - 1)
+                 dep_a_src=None if T is None else len(srcs) - 1, **self._merged_tiling(M, N, prog))
         if save is not None:
             save.append(LinearRec("linear", name, xl, T))
         return out
@@ -600,8 +632,12 @@ class UNetB200:
         C = sum(x.shape[-1] for x in xs)
         out = self._new(B * HW, C)
         stats = self._new(B, self.cfg.norm_num_groups, 2, dtype=torch.float32)
-        ops.groupnorm_fwd(xs[0], xs[1] if len(xs) > 1 else None, L.gamma, L.beta, eps, silu, out, stats,
-                          B, HW, self.cfg.norm_num_groups)
+        x2 = xs[1] if len(xs) > 1 else None
+        if self._plan_b is None:
+            ops.groupnorm_fwd(xs[0], x2, L.gamma, L.beta, eps, silu, out, stats, B, HW, self.cfg.norm_num_groups)
+        else:   # a rebuilt block: merge each image's statistics from the merged pass's partition
+            ops.groupnorm_fwd_part(xs[0], x2, L.gamma, L.beta, eps, silu, out, stats, B, self._plan_b, HW,
+                                   self.cfg.norm_num_groups)
         if save is not None:
             lb = self._lrows(B)
             save.append(GNRec("gn", name, xs if lb == B else [x[:lb * HW] for x in xs], stats[:lb], eps, silu, lb, HW))
@@ -719,6 +755,14 @@ class UNetB200:
             out = self.conv3(name, [xu], lora, save=s)
         return out, ResampleRec(name, _last(s), up)
 
+    def _block(self, kind, name, xs, st, ctx, lora, save, up=False):
+        """One block's forward: (out, record)."""
+        if kind == "resnet":
+            return self.resnet(name, xs, st, lora, save)
+        if kind == "transformer":
+            return self.transformer(name, xs[0], ctx, lora, save)
+        return self.resample(name, xs[0], lora, save, up)
+
     def _lrows(self, n):
         """Rows / samples of an n-row (batch-major) tensor that belong to the LoRA samples."""
         lb, bt = self._lb
@@ -734,7 +778,14 @@ class UNetB200:
         lora_batch = b < B runs ONE pass in which only the first b samples carry the LoRA adapter
         (student) and the rest see the frozen base weights (teacher): the adapter's T = A(x) is computed
         for the leading rows only and the fused LoRA K-block reads zeros for the others.  The tape then
-        holds views of the first b samples, so backward() is the student's backward."""
+        holds views of the first b samples, so backward() is the student's backward.
+
+        With gradient_checkpointing, save=True keeps a CheckpointRec per block instead: owned copies of
+        the student rows of the block's inputs (one copy per tensor: a down-path output that is the next
+        block's input and a skip is kept once), so the merged pass's activations and every block-internal
+        tensor are freed as the forward proceeds.  The time-embedding and context projections of the pass
+        stay referenced (small), and the head's GroupNorm record keeps a copy of its student rows.
+        backward() then rebuilds one block's full record at a time."""
         cfg = self.cfg
         lora = lora and self.has_lora
         B, H, W, _ = sample.shape
@@ -770,10 +821,27 @@ class UNetB200:
         Lci = self.layers["conv_in"]
         ops.conv3x3_c4(sample, Lci.w_c4, Lci.bias, x, sgn=1, round_in=True)
         tape, skips = [], [x]       # tape: the block records in forward order
+        ck = save and self.gradient_checkpointing
+        lb = self._lb[0]
+        copies = {}                 # checkpointing: id of a block input -> (weak reference, its copy)
 
-        def run(out_rec):
-            tape.append(out_rec[1])
-            return out_rec[0]
+        def student_rows(xs):
+            out = []
+            for t in xs:
+                hit = copies.get(id(t))
+                if hit is None or hit[0]() is not t:
+                    hit = (weakref.ref(t), t if lb == B else t[:lb].clone())
+                    copies[id(t)] = hit
+                out.append(hit[1])
+            return out
+
+        def run(kind, name, xs, up=False):
+            if ck:
+                tape.append(CheckpointRec(kind, name, student_rows(xs), len(xs) == 2, up))
+                return self._block(kind, name, xs, st, ctx, lora, False, up)[0]
+            out, rec = self._block(kind, name, xs, st, ctx, lora, save, up)
+            tape.append(rec)
+            return out
 
         def push(x):                # the last block's output x becomes a skip input of the up path
             tape[-1].pushes_skip = True
@@ -782,30 +850,61 @@ class UNetB200:
         nb = len(cfg.block_out_channels)
         for i in range(nb):
             for j in range(cfg.layers_per_block):
-                x = run(self.resnet(f"down_blocks.{i}.resnets.{j}", [x], st, lora, save))
+                x = run("resnet", f"down_blocks.{i}.resnets.{j}", [x])
                 if cfg.down_attn[i]:
-                    x = run(self.transformer(f"down_blocks.{i}.attentions.{j}", x, ctx, lora, save))
+                    x = run("transformer", f"down_blocks.{i}.attentions.{j}", [x])
                 push(x)
             if i < nb - 1:
-                x = run(self.resample(f"down_blocks.{i}.downsamplers.0.conv", x, lora, save, up=False))
+                x = run("resample", f"down_blocks.{i}.downsamplers.0.conv", [x])
                 push(x)
-        x = run(self.resnet("mid_block.resnets.0", [x], st, lora, save))
-        x = run(self.transformer("mid_block.attentions.0", x, ctx, lora, save))
-        x = run(self.resnet("mid_block.resnets.1", [x], st, lora, save))
+        x = run("resnet", "mid_block.resnets.0", [x])
+        x = run("transformer", "mid_block.attentions.0", [x])
+        x = run("resnet", "mid_block.resnets.1", [x])
         for i in range(nb):
             for j in range(cfg.layers_per_block + 1):
-                x = run(self.resnet(f"up_blocks.{i}.resnets.{j}", [x, skips.pop()], st, lora, save))
+                x = run("resnet", f"up_blocks.{i}.resnets.{j}", [x, skips.pop()])
                 if cfg.up_attn[i]:
-                    x = run(self.transformer(f"up_blocks.{i}.attentions.{j}", x, ctx, lora, save))
+                    x = run("transformer", f"up_blocks.{i}.attentions.{j}", [x])
             if i < nb - 1:
-                x = run(self.resample(f"up_blocks.{i}.upsamplers.0.conv", x, lora, save, up=True))
+                x = run("resample", f"up_blocks.{i}.upsamplers.0.conv", [x], up=True)
         Bx, Hx, Wx, Cx = x.shape
         head = [] if save else None
         g = self.gn("conv_norm_out", [x.view(Bx * Hx * Wx, Cx)], Bx, Hx * Wx, 1e-5, True, head)
         eps = self.conv3("conv_out", [g.view(Bx, Hx, Wx, Cx)], False, out_fp32=True)
         if save:
-            self.saved = (tape, head[0], (self._lb[0], H, W))
+            rebuild = None
+            if ck:
+                h = head[0]      # already the student rows: views of the merged pass's last activation
+                if lb != B:
+                    head[0] = h._replace(xs=[t.clone() for t in h.xs], stats=h.stats.clone())
+                rebuild = self._rebuild_state(lora, B, st, ctx)
+            self.saved = (tape, head[0], (lb, H, W), rebuild)
         return eps
+
+    def _rebuild_state(self, lora, B, st, ctx):
+        """What rebuilding a checkpointed block of this pass needs besides its inputs: the student rows of
+        the pass's time embedding, of its grouped time_emb_proj output and of its context k / v."""
+        lb = self._lb[0]
+        out_all, T = self._temb
+        kv = self._ctxkv
+        S = ctx.shape[0] // B
+        if kv is not None:
+            kv = {t: (k[:lb * S], v[:lb * S], Tkv) for t, (k, v, Tkv) in kv.items()}
+        return types.SimpleNamespace(lora=lora, B=B, lb=lb, st=st[:lb], ctx=ctx[:lb * S], temb=(out_all[:lb], T),
+                                     ctxkv=kv)
+
+    def _rebuild(self, ck, state):
+        """The full record of a checkpointed block: its forward once more, on the saved student rows, with
+        the launch plans of the merged pass that first ran it, so that every tensor of the record is
+        bitwise the one the stored tape would hold."""
+        prev = self._lb, self._temb, self._ctxkv
+        self._lb, self._temb, self._ctxkv = (state.lb, state.lb), state.temb, state.ctxkv
+        self._plan_b = state.B if state.B != state.lb else None
+        try:
+            return self._block(ck.kind, ck.name, ck.xs, state.st, state.ctx, state.lora, True, ck.up)[1]
+        finally:
+            self._lb, self._temb, self._ctxkv = prev
+            self._plan_b = None
 
     # ------------------------------------------------------------------------------------
     # backward primitives
@@ -1048,7 +1147,7 @@ class UNetB200:
         Accumulates LoRA gradients into self.lora_grad (caller zeroes it between steps).
         grad_ready(offset): called (on the weight-gradient stream) after each block's backward with
         the flat-buffer offset from which every gradient element is final."""
-        tape, head, (B, H, W) = self.saved
+        tape, head, (B, H, W), rebuild = self.saved
         self._dkv_chunks = {}
         boffs = self.block_grad_offsets() if grad_ready is not None else None
         Lco = self.layers["conv_out"]
@@ -1059,6 +1158,7 @@ class UNetB200:
         d = d.view(B, H, W, c0)
         dskips = []     # gradients of the up path's skip inputs; the last one left (conv_in's output) is unused
         done = None     # the block walked before the current one
+        side = []       # checkpointing: (event, tensors) of the weight-gradient work of the last blocks walked
         for i in reversed(range(len(tape))):
             blk = tape[i]
             if blk.pushes_skip:
@@ -1068,6 +1168,9 @@ class UNetB200:
             if grad_ready is not None and boffs.get(done) is not None:
                 with UNetB200._Side(self, ()):
                     grad_ready(boffs[done])
+            if isinstance(blk, CheckpointRec):
+                tape[i] = None              # the rebuilt record holds what the backward still reads
+                blk = self._rebuild(blk, rebuild)
             if isinstance(blk, ResnetRec):
                 d, dskip = self.resnet_bwd(blk, d, need_dx=i > 0)
                 if blk.takes_skip:
@@ -1077,8 +1180,27 @@ class UNetB200:
             else:
                 d = self.resample_bwd(blk, d)
             done = blk.name
+            if rebuild is not None:
+                self._release_side(side)
         if grad_ready is not None:
             with UNetB200._Side(self, ()):
                 grad_ready(0)
         self._join_side()
+        side.clear()
         self.saved = None
+
+    def _release_side(self, side):
+        """Checkpointing: the tensors the weight-gradient stream reads stay referenced (_Side keeps them)
+        until that stream is done with them.  Joining the streams after every block would serialise the
+        weight gradients with the backward chain, so release them one block late: the current stream
+        waits for the side work of the block walked before this one, which has had a whole block's
+        backward to finish, and then drops its tensors."""
+        if not self.use_wstream:
+            return
+        ev = torch.cuda.Event()
+        ev.record(self.wstream)
+        side.append((ev, self._keep))
+        self._keep = []
+        if len(side) > 1:
+            ev, _ = side.pop(0)
+            torch.cuda.current_stream().wait_event(ev)
