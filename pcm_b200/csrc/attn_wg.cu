@@ -20,7 +20,8 @@ namespace pcm {
 namespace {
 
 constexpr int kAwThreads = 384;
-constexpr int kAwStages = 2;
+constexpr int kAwStages = 2;    // K / V ring of the forward
+constexpr int kBwdStages = 3;   // streamed Q / dO or K / V ring of the backward
 constexpr int kTile = 64 * 128;  // 64 rows x 64 bf16, SWIZZLE_128B
 
 struct alignas(64) AttnWgParams {
@@ -31,6 +32,20 @@ struct alignas(64) AttnWgParams {
   long long ldo;
   float c;  // scale * log2(e)
 };
+
+// Keep a register A operand of an in-flight wgmma live and unchanged until its group has been waited for.
+__device__ __forceinline__ void keep_operand(uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) asm volatile("" : "+r"(a[i][k])::"memory");
+}
+
+// P (fp32, in the accumulator fragment) -> bf16 register A operands of 4 k-steps of 16 keys
+__device__ __forceinline__ void pack_operand(uint32_t (&a)[4][4], const float (&x)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) a[i >> 3][(i & 7) >> 1] = pack_bf16x2(x[i], x[i + 1]);
+}
 
 template <int KB>
 __global__ void __launch_bounds__(kAwThreads, 1) attn_fwd_wg_kernel(const __grid_constant__ AttnWgParams p) {
@@ -164,7 +179,7 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_fwd_wg_kernel(const __grid
     for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
       for (int kb = 0; kb < KB; ++kb)   // V: 16 keys x 64 head columns, MN-major
-        wgmma_rs_m64n64<1>(o[kb], pa[kk], wgmma_desc_sw128(v_addr + kb * kTile + kk * 2048, kTile, 1024), 1u);
+        WgmmaRs<64, 1>::mma(o[kb], pa[kk], wgmma_desc_sw128(v_addr + kb * kTile + kk * 2048, kTile, 1024), 1u);
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
@@ -209,6 +224,12 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_fwd_wg_kernel(const __grid
 // A operand of the RS-form wgmma against the streamed tile read MN-major, as in the forward.  The
 // columns past d of the resident tiles are zeroed, so the next head's columns that the 64-wide boxes
 // also cover add nothing; keys past Skv are masked, queries past Sq have L = +inf (P = 0).
+// For d <= 40 only what the head needs is multiplied: S and dP contract over 3 k-steps (48 columns, the
+// zeroed ones past d included) and the accumulators hold 40 columns (NV = 40).  The dropped k-step only
+// added products with zeroed columns and the dropped columns were never stored, so the results are
+// those of the 64-column products bit for bit.
+// Pipeline: block j's S / dP products are issued ahead of block j-1's accumulator products, and block
+// j's elementwise P / dS work runs while the latter are on the tensor cores.
 // ------------------------------------------------------------------------------------------
 struct alignas(64) AttnBwdParams {
   CUtensorMap fix0_map, fix1_map;   // resident tiles: K, V (KV) or Q, dO
@@ -221,16 +242,51 @@ struct alignas(64) AttnBwdParams {
   float c, scale;
 };
 
-template <bool KV>
+// P and dS of one 64-column block, in place: s becomes P, dp becomes dS (fp32).  KV: row = key (valid
+// per row), the column statistics lc / dc were loaded for this block; dQ: column = key, MASK when the
+// block's keys from kcol on may lie past Skv.
+template <bool KV, bool MASK>
+__device__ __forceinline__ void bwd_elementwise(float (&s)[32], float (&dp)[32], const float (&lc)[16],
+                                                const float (&dc)[16], const float (&lrow)[2],
+                                                const float (&drow)[2], const bool (&rvalid)[2], float c,
+                                                int kcol, int Skv) {
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int r = (i >> 1) & 1;
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float l, d;
+      bool ok;
+      if (KV) {
+        l = lc[2 * (i >> 2) + e];
+        d = dc[2 * (i >> 2) + e];
+        ok = rvalid[r];
+      } else {
+        l = lrow[r];
+        d = drow[r];
+        ok = !MASK || kcol + 8 * (i >> 2) + e < Skv;
+      }
+      const float pv = ok ? exp2f(s[i + e] * c - l) : 0.f;
+      s[i + e] = pv;
+      dp[i + e] = pv * (dp[i + e] - d);
+    }
+  }
+}
+
+template <bool KV, int NV>
 __global__ void __launch_bounds__(kAwThreads, 1) attn_bwd_wg_kernel(const __grid_constant__ AttnBwdParams p) {
+  constexpr int kStages = kBwdStages;
+  constexpr int KS = (NV + 15) / 16;   // k-steps of S / dP
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* sF = smem;                          // [2 warpgroups][2 tiles]
   uint8_t* sS = sF + 4 * kTile;                // [stages][2 tiles]
   __shared__ __align__(8) uint64_t f_bar;
-  __shared__ __align__(8) uint64_t full_bar[kAwStages];
-  __shared__ __align__(8) uint64_t empty_bar[kAwStages];
+  __shared__ __align__(8) uint64_t full_bar[kStages];
+  __shared__ __align__(8) uint64_t empty_bar[kStages];
+  // (KV) L and delta of the streamed query block, per consumer warpgroup, double-buffered
+  __shared__ float stats[2][2][2][64];   // [warpgroup][buffer][L, delta][query]
 
   const int wg = threadIdx.x >> 7;
   const int b = blockIdx.z, h = blockIdx.y, r0 = blockIdx.x * 128;
@@ -243,7 +299,7 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_bwd_wg_kernel(const __grid
     tma_prefetch_desc(&p.str0_map);
     tma_prefetch_desc(&p.str1_map);
     mbar_init(&f_bar, 1);
-    for (int i = 0; i < kAwStages; ++i) {
+    for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 2);
     }
@@ -261,8 +317,8 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_bwd_wg_kernel(const __grid
         tma_load_3d(sF + (2 * w + 1) * kTile, &p.fix1_map, &f_bar, col0, r0 + 64 * w, b);
       }
       for (int j = 0; j < nblk; ++j) {
-        const int st = j % kAwStages;
-        mbar_wait(&empty_bar[st], ((j / kAwStages) & 1) ^ 1);
+        const int st = j % kStages;
+        mbar_wait(&empty_bar[st], ((j / kStages) & 1) ^ 1);
         mbar_arrive_expect_tx(&full_bar[st], 2 * kTile);
         tma_load_3d(sS + (2 * st) * kTile, &p.str0_map, &full_bar[st], col0, j * 64, b);
         tma_load_3d(sS + (2 * st + 1) * kTile, &p.str1_map, &full_bar[st], col0, j * 64, b);
@@ -300,79 +356,108 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_bwd_wg_kernel(const __grid
       drow[r] = rvalid[r] ? Dl[frow + 8 * r] : 0.f;
     }
   }
-  float acc0[32], acc1[32];   // KV: dK, dV;  dQ: dQ (acc1 unused)
+  float acc0[NV / 2], acc1[NV / 2];   // KV: dK, dV;  dQ: dQ (acc1 unused)
 #pragma unroll
-  for (int i = 0; i < 32; ++i) acc0[i] = acc1[i] = 0.f;
+  for (int i = 0; i < NV / 2; ++i) acc0[i] = acc1[i] = 0.f;
   const uint32_t f0 = smem_u32(myF), f1 = f0 + kTile;
+  const bool ragged = !KV && (p.Skv & 63) != 0;
+  float s[32], dp[32];
+  uint32_t pa[4][4], dsa[4][4];         // P^T / dS of the previous block as register A operands
 
-  for (int j = 0; j < nblk; ++j) {
-    const int st = j % kAwStages;
-    mbar_wait(&full_bar[st], (j / kAwStages) & 1);
+  auto issue_sdp = [&](int st) {
     const uint32_t s0 = smem_u32(sS + 2 * st * kTile), s1 = s0 + kTile;
-    float s[32], dp[32];
-    wgmma_fence();
+    Wgmma<64, 0, 0>::mma_first(s, wgmma_desc_sw128(f0, 16, 1024), wgmma_desc_sw128(s0, 16, 1024));
+    Wgmma<64, 0, 0>::mma_first(dp, wgmma_desc_sw128(f1, 16, 1024), wgmma_desc_sw128(s1, 16, 1024));
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      Wgmma<64, 0, 0>::mma(s, wgmma_desc_sw128(f0 + k * 32, 16, 1024), wgmma_desc_sw128(s0 + k * 32, 16, 1024),
-                           k != 0 ? 1u : 0u);
-      Wgmma<64, 0, 0>::mma(dp, wgmma_desc_sw128(f1 + k * 32, 16, 1024), wgmma_desc_sw128(s1 + k * 32, 16, 1024),
-                           k != 0 ? 1u : 0u);
+    for (int k = 1; k < KS; ++k) {
+      Wgmma<64, 0, 0>::mma(s, wgmma_desc_sw128(f0 + k * 32, 16, 1024), wgmma_desc_sw128(s0 + k * 32, 16, 1024), 1u);
+      Wgmma<64, 0, 0>::mma(dp, wgmma_desc_sw128(f1 + k * 32, 16, 1024), wgmma_desc_sw128(s1 + k * 32, 16, 1024), 1u);
     }
     wgmma_commit();
-    // (KV) statistics of this block's 16 query columns of the thread, loaded while the MMAs run
-    float lc[16], dc[16];
-    if (KV) {
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int qi = j * 64 + 8 * q + 2 * (lane & 3) + e;
-          lc[2 * q + e] = qi < p.Sq ? L[qi] : INFINITY;
-          dc[2 * q + e] = qi < p.Sq ? Dl[qi] : 0.f;
-        }
-    }
-    wgmma_wait<0>();
-    wgmma_fence_acc(s);
-    wgmma_fence_acc(dp);
-    uint32_t pa[4][4], dsa[4][4];
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const int r = (i >> 1) & 1;
-      float pv[2], g[2];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int col = 8 * (i >> 2) + 2 * (lane & 3) + e;   // column of the score tile in this block
-        float l, d;
-        bool ok;
-        if (KV) {
-          l = lc[2 * (i >> 2) + e];
-          d = dc[2 * (i >> 2) + e];
-          ok = rvalid[r];                 // row = key
-        } else {
-          l = lrow[r];
-          d = drow[r];
-          ok = j * 64 + col < p.Skv;      // column = key
-        }
-        pv[e] = ok ? exp2f(s[i + e] * p.c - l) : 0.f;
-        g[e] = pv[e] * (dp[i + e] - d);
-      }
-      pa[i >> 3][(i & 7) >> 1] = pack_bf16x2(pv[0], pv[1]);
-      dsa[i >> 3][(i & 7) >> 1] = pack_bf16x2(g[0], g[1]);
-    }
-    wgmma_fence();
+  };
+  auto issue_acc = [&](int st) {
+    const uint32_t s0 = smem_u32(sS + 2 * st * kTile), s1 = s0 + kTile;
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
-      // streamed tile 0 (Q for dK, K for dQ) and 1 (dO for dV), 16 rows x 64 columns, MN-major
-      wgmma_rs_m64n64<1>(acc0, dsa[kk], wgmma_desc_sw128(s0 + kk * 2048, kTile, 1024), 1u);
-      if (KV) wgmma_rs_m64n64<1>(acc1, pa[kk], wgmma_desc_sw128(s1 + kk * 2048, kTile, 1024), 1u);
+      // streamed tile 0 (Q for dK, K for dQ) and 1 (dO for dV), 16 rows x NV columns, MN-major
+      WgmmaRs<NV, 1>::mma(acc0, dsa[kk], wgmma_desc_sw128(s0 + kk * 2048, kTile, 1024), 1u);
+      if (KV) WgmmaRs<NV, 1>::mma(acc1, pa[kk], wgmma_desc_sw128(s1 + kk * 2048, kTile, 1024), 1u);
     }
     wgmma_commit();
+  };
+  // (KV) the L / delta of query block j: one value per thread, loaded a block ahead of its use (the
+  // load runs under the block's MMAs and elementwise work), published through shared memory
+  auto load_stat = [&](int j) {
+    const int qi = j * 64 + (et & 63);
+    if (et < 64) return qi < p.Sq ? L[qi] : INFINITY;
+    return qi < p.Sq ? Dl[qi] : 0.f;
+  };
+  auto publish_stat = [&](int j, float v) {
+    stats[cw][j & 1][et >> 6][et & 63] = v;
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+  };
+  auto elementwise = [&](int j) {
+    const int kcol = j * 64 + 2 * (lane & 3);
+    float lc[16], dc[16];   // (KV) statistics of the block's 16 query columns of the thread
+    if (KV) {
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float2 l2 = *reinterpret_cast<const float2*>(&stats[cw][j & 1][0][8 * q + 2 * (lane & 3)]);
+        const float2 d2 = *reinterpret_cast<const float2*>(&stats[cw][j & 1][1][8 * q + 2 * (lane & 3)]);
+        lc[2 * q] = l2.x;
+        lc[2 * q + 1] = l2.y;
+        dc[2 * q] = d2.x;
+        dc[2 * q + 1] = d2.y;
+      }
+    }
+    if (ragged && j == nblk - 1)
+      bwd_elementwise<KV, true>(s, dp, lc, dc, lrow, drow, rvalid, p.c, kcol, p.Skv);
+    else
+      bwd_elementwise<KV, false>(s, dp, lc, dc, lrow, drow, rvalid, p.c, kcol, p.Skv);
+  };
+
+  if (KV) publish_stat(0, load_stat(0));
+  mbar_wait(&full_bar[0], 0);
+  wgmma_fence();
+  issue_sdp(0);
+  float nxt = KV ? load_stat(1) : 0.f;
+  wgmma_wait<0>();
+  wgmma_fence_acc(s);
+  wgmma_fence_acc(dp);
+  elementwise(0);
+  if (KV) publish_stat(1, nxt);
+  pack_operand(pa, s);
+  pack_operand(dsa, dp);
+
+  for (int j = 1; j < nblk; ++j) {
+    const int st = j % kStages, pst = (j - 1) % kStages;
+    mbar_wait(&full_bar[st], (j / kStages) & 1);
+    wgmma_fence();
+    issue_sdp(st);       // S_j, dP_j ...
+    issue_acc(pst);      // ... then the accumulator products of block j-1
+    if (KV) nxt = load_stat(j + 1);
+    wgmma_wait<1>();     // S_j and dP_j have landed
+    wgmma_fence_acc(s);
+    wgmma_fence_acc(dp);
+    elementwise(j);
+    if (KV) publish_stat(j + 1, nxt);
     wgmma_wait<0>();
     wgmma_fence_acc(acc0);
     wgmma_fence_acc(acc1);
+    keep_operand(pa);
+    keep_operand(dsa);
     __syncwarp();
-    if (et == 0) mbar_arrive(&empty_bar[st]);
+    if (et == 0) mbar_arrive(&empty_bar[pst]);
+    pack_operand(pa, s);
+    pack_operand(dsa, dp);
   }
+  wgmma_fence();
+  issue_acc((nblk - 1) % kStages);
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc0);
+  wgmma_fence_acc(acc1);
+  keep_operand(pa);
+  keep_operand(dsa);
 
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -381,7 +466,7 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_bwd_wg_kernel(const __grid
     bf16* o0 = p.out0 + row * p.ld0 + col0;
     bf16* o1 = KV ? p.out1 + row * p.ld1 + col0 : nullptr;
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
+    for (int q = 0; q < NV / 8; ++q) {
       const int col = 8 * q + 2 * (lane & 3);
       if (col < p.D) {
         *reinterpret_cast<uint32_t*>(o0 + col) =
@@ -402,6 +487,19 @@ int encode_seq_map(CUtensorMap* m, const void* base, int HD, int S, int B, long 
   cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * 2, static_cast<cuuint64_t>(ld) * 2 * S};
   cuuint32_t box[3] = {64, 64, 1}, estr[3] = {1, 1, 1};
   return encode_tmap(m, base, 3, dims, strides, box, estr);
+}
+
+template <bool KV, int NV>
+cudaError_t launch_bwd(dim3 grid, cudaStream_t stream, const AttnBwdParams& p) {
+  const size_t smem = (4 + 2 * kBwdStages) * kTile + 1024;
+  static bool attr = false;
+  if (!attr) {
+    const cudaError_t e = cudaFuncSetAttribute(attn_bwd_wg_kernel<KV, NV>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               static_cast<int>(smem));
+    if (e != cudaSuccess) return e;
+    attr = true;
+  }
+  return launch_pdl(attn_bwd_wg_kernel<KV, NV>, grid, dim3(kAwThreads), smem, stream, p);
 }
 
 }  // namespace
@@ -472,17 +570,14 @@ int attn_bwd_wg(const void* q, const void* k, const void* v, const void* dout, c
   pq.out0 = reinterpret_cast<bf16*>(dq); pq.ld0 = ldq;
   pq.out1 = nullptr; pq.ld1 = 0;
   pq.n_fix = Sq; pq.n_str = Skv; pq.scale = scale;
-  const size_t smem = (4 + 2 * kAwStages) * kTile + 1024;
-  static bool attr = false;
-  if (!attr) {
-    CUDA_TRY(cudaFuncSetAttribute(attn_bwd_wg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(smem)));
-    CUDA_TRY(cudaFuncSetAttribute(attn_bwd_wg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(smem)));
-    attr = true;
+  const dim3 gk((Skv + 127) / 128, H, B), gq((Sq + 127) / 128, H, B);
+  if (D <= 40) {
+    CUDA_TRY((launch_bwd<true, 40>)(gk, stream, pk));
+    CUDA_TRY((launch_bwd<false, 40>)(gq, stream, pq));
+  } else {
+    CUDA_TRY((launch_bwd<true, 64>)(gk, stream, pk));
+    CUDA_TRY((launch_bwd<false, 64>)(gq, stream, pq));
   }
-  CUDA_TRY(launch_pdl(attn_bwd_wg_kernel<true>, dim3((Skv + 127) / 128, H, B), dim3(kAwThreads), smem, stream, pk));
-  CUDA_TRY(launch_pdl(attn_bwd_wg_kernel<false>, dim3((Sq + 127) / 128, H, B), dim3(kAwThreads), smem, stream, pq));
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
