@@ -163,15 +163,15 @@ __global__ void __launch_bounds__(256) attn_fwd_kernel(const AttnParams p) {
       mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
       mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
       const float mn = fmaxf(m_run[r], mx[r]);
-      alpha[r] = exp2f(m_run[r] - mn);
+      alpha[r] = exp2_ftz(m_run[r] - mn);
       m_run[r] = mn;
     }
     float rs[2] = {0.f, 0.f};
     uint32_t pa[4][4];  // P as A fragments for 4 k-steps of 16 keys
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      const float p0 = exp2f(s[i][0] - m_run[0]), p1 = exp2f(s[i][1] - m_run[0]);
-      const float p2 = exp2f(s[i][2] - m_run[1]), p3 = exp2f(s[i][3] - m_run[1]);
+      const float p0 = exp2_ftz(s[i][0] - m_run[0]), p1 = exp2_ftz(s[i][1] - m_run[0]);
+      const float p2 = exp2_ftz(s[i][2] - m_run[1]), p3 = exp2_ftz(s[i][3] - m_run[1]);
       rs[0] += p0 + p1;
       rs[1] += p2 + p3;
       pa[i >> 1][(i & 1) * 2] = pack_bf16x2(p0, p1);
@@ -339,10 +339,10 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnParams p) 
       const float l0 = sLs[qc], l1 = sLs[qc + 1];
       const float d0 = sDs[qc], d1 = sDs[qc + 1];
       float pv[4];
-      pv[0] = kvalid[0] ? exp2f(s[i][0] * c - l0) : 0.f;
-      pv[1] = kvalid[0] ? exp2f(s[i][1] * c - l1) : 0.f;
-      pv[2] = kvalid[1] ? exp2f(s[i][2] * c - l0) : 0.f;
-      pv[3] = kvalid[1] ? exp2f(s[i][3] * c - l1) : 0.f;
+      pv[0] = kvalid[0] ? exp2_ftz(__fmaf_rn(s[i][0], c, -l0)) : 0.f;
+      pv[1] = kvalid[0] ? exp2_ftz(__fmaf_rn(s[i][1], c, -l1)) : 0.f;
+      pv[2] = kvalid[1] ? exp2_ftz(__fmaf_rn(s[i][2], c, -l0)) : 0.f;
+      pv[3] = kvalid[1] ? exp2_ftz(__fmaf_rn(s[i][3], c, -l1)) : 0.f;
       const float g0 = pv[0] * (dp[i][0] - d0), g1 = pv[1] * (dp[i][1] - d1);
       const float g2 = pv[2] * (dp[i][2] - d0), g3 = pv[3] * (dp[i][3] - d1);
       pa[i >> 1][(i & 1) * 2] = pack_bf16x2(pv[0], pv[1]);
@@ -464,7 +464,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnParams p) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int key = kbase + i * 8 + (e & 1);
-        const float pv = key < p.Skv ? exp2f(s[i][e] * c - lrow[e >> 1]) : 0.f;
+        const float pv = key < p.Skv ? exp2_ftz(__fmaf_rn(s[i][e], c, -lrow[e >> 1])) : 0.f;
         g[e] = pv * (dp[i][e] - drow[e >> 1]);
       }
       dsa[i >> 1][(i & 1) * 2] = pack_bf16x2(g[0], g[1]);

@@ -7,10 +7,12 @@
 // TMA wrote.  Head columns are handled in 64-wide blocks (KB = 1 for d <= 64, 2 for d <= 128); the
 // columns of a block past d belong to the next head (or lie outside the tensor map and read as zero):
 // they are zeroed in Q, so they add nothing to S, and the matching O columns are not stored.
-// Keys past Skv (zero rows of the tensor map) are masked to -inf.
+// Keys past Skv (zero rows of the tensor map) are masked to -inf in the last block of a ragged Skv.
 //
 // Same contract as attn_fwd_kernel (attn.cu): q [B, Sq, H*D] (row stride ldq), k / v [B, Skv, H*D],
 // out like q, lse [B, H, Sq] in log2 units of the scaled scores.
+#include <type_traits>
+
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "host_common.h"
@@ -47,8 +49,49 @@ __device__ __forceinline__ void pack_operand(uint32_t (&a)[4][4], const float (&
   for (int i = 0; i < 32; i += 2) a[i >> 3][(i & 7) >> 1] = pack_bf16x2(x[i], x[i + 1]);
 }
 
-template <int KB>
+// Online softmax of one 64-key block on the S accumulator fragment (rows r and r + 8 of the thread; a
+// row lives in one quad of lanes).  s becomes c S, with keys from kbase on past Skv at -inf when MASK;
+// m_run takes the block's row maxima, alpha the factors that rescale the old row state, rs the block's
+// row sums of P = exp2(c S - m), and pa P as register A operands of 4 k-steps of 16 keys.
+// The scale and the subtraction round separately (no FFMA), as they did when the mask's select stood
+// between them; exp2_ftz only drops P / alpha below 2^-126, weights that cannot move a row sum whose
+// largest term is 1.
+template <bool MASK>
+__device__ __forceinline__ void fwd_softmax(float (&s)[32], float (&m_run)[2], float (&alpha)[2], float (&rs)[2],
+                                            uint32_t (&pa)[4][4], float c, int kbase, int Skv) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    float v = __fmul_rn(s[i], c);
+    if (MASK && kbase + 8 * (i >> 2) + (i & 1) >= Skv) v = -INFINITY;
+    s[i] = v;
+    mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+    const float mn = fmaxf(m_run[r], mx[r]);
+    alpha[r] = exp2_ftz(m_run[r] - mn);
+    m_run[r] = mn;
+    rs[r] = 0.f;
+  }
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int r = (i >> 1) & 1;
+    const float p0 = exp2_ftz(__fsub_rn(s[i], m_run[r])), p1 = exp2_ftz(__fsub_rn(s[i + 1], m_run[r]));
+    rs[r] += p0 + p1;
+    pa[i >> 3][(i & 7) >> 1] = pack_bf16x2(p0, p1);
+  }
+}
+
+// KB 64-column blocks of head columns; NV = 40 (KB = 1, d <= 40) multiplies only what the head needs, as
+// the backward does: S contracts over 3 k-steps (48 columns, the zeroed ones past d included) and O holds
+// 40 columns, bitwise the results of the 64-column products.
+template <int KB, int NV>
 __global__ void __launch_bounds__(kAwThreads, 1) attn_fwd_wg_kernel(const __grid_constant__ AttnWgParams p) {
+  static_assert(NV == 64 || (KB == 1 && NV == 40), "trimmed products only for one 64-column block");
+  constexpr int KS = (NV + 15) / 16;   // k-steps of S per 64-column block
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -114,15 +157,16 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_fwd_wg_kernel(const __grid
   }
   asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
 
-  float o[KB][32];
+  float o[KB][NV / 2];
 #pragma unroll
   for (int kb = 0; kb < KB; ++kb)
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[kb][i] = 0.f;
+    for (int i = 0; i < NV / 2; ++i) o[kb][i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   const uint32_t q_addr = smem_u32(myQ);
 
-  for (int j = 0; j < nblk; ++j) {
+  // one 64-key block; MASK only for the last block of a ragged Skv (the keys past Skv read as zero rows)
+  auto block = [&](int j, auto mask) {
     const int st = j % kAwStages;
     mbar_wait(&full_bar[st], (j / kAwStages) & 1);
     const uint32_t k_addr = smem_u32(sK + st * KB * kTile);
@@ -132,61 +176,43 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_fwd_wg_kernel(const __grid
 #pragma unroll
     for (int kb = 0; kb < KB; ++kb)
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
+      for (int k = 0; k < KS; ++k)
         Wgmma<64, 0, 0>::mma(s, wgmma_desc_sw128(q_addr + kb * kTile + k * 32, 16, 1024),
                              wgmma_desc_sw128(k_addr + kb * kTile + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(s);
 
-    // scale, mask, online softmax (rows r and r + 8 of the thread; a row lives in one quad of lanes)
-    const int kbase = j * 64 + 2 * (lane & 3);
-    float mx[2] = {-INFINITY, -INFINITY};
+    float alpha[2], rs[2];
+    uint32_t pa[4][4];
+    fwd_softmax<decltype(mask)::value>(s, m_run, alpha, rs, pa, p.c, j * 64 + 2 * (lane & 3), p.Skv);
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int key = kbase + 8 * (i >> 2) + (i & 1);
-      const float v = key < p.Skv ? s[i] * p.c : -INFINITY;
-      s[i] = v;
-      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
+    for (int r = 0; r < 2; ++r) l_run[r] = __fmaf_rn(l_run[r], alpha[r], rs[r]);
+    // alpha = 1 where the row maximum did not change: when it holds for every row of the warp, the
+    // rescale (an exact multiply by 1) is skipped
+    if (!__all_sync(0xffffffffu, alpha[0] == 1.f && alpha[1] == 1.f)) {
+#pragma unroll
+      for (int kb = 0; kb < KB; ++kb)
+#pragma unroll
+        for (int i = 0; i < NV / 2; ++i) o[kb][i] *= alpha[(i >> 1) & 1];
     }
-    float alpha[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float mn = fmaxf(m_run[r], mx[r]);
-      alpha[r] = exp2f(m_run[r] - mn);
-      m_run[r] = mn;
-    }
-    float rs[2] = {0.f, 0.f};
-    uint32_t pa[4][4];  // P as register A operands of 4 k-steps of 16 keys
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const int r = (i >> 1) & 1;
-      const float p0 = exp2f(s[i] - m_run[r]), p1 = exp2f(s[i + 1] - m_run[r]);
-      rs[r] += p0 + p1;
-      pa[i >> 3][(i & 7) >> 1] = pack_bf16x2(p0, p1);
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + rs[r];
-#pragma unroll
-    for (int kb = 0; kb < KB; ++kb)
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o[kb][i] *= alpha[(i >> 1) & 1];
 
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
-      for (int kb = 0; kb < KB; ++kb)   // V: 16 keys x 64 head columns, MN-major
-        WgmmaRs<64, 1>::mma(o[kb], pa[kk], wgmma_desc_sw128(v_addr + kb * kTile + kk * 2048, kTile, 1024), 1u);
+      for (int kb = 0; kb < KB; ++kb)   // V: 16 keys x NV head columns, MN-major
+        WgmmaRs<NV, 1>::mma(o[kb], pa[kk], wgmma_desc_sw128(v_addr + kb * kTile + kk * 2048, kTile, 1024), 1u);
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
     for (int kb = 0; kb < KB; ++kb) wgmma_fence_acc(o[kb]);
     __syncwarp();
     if (et == 0) mbar_arrive(&empty_bar[st]);
-  }
+  };
+  const int nfull = p.Skv / 64;
+  for (int j = 0; j < nfull; ++j) block(j, std::false_type());
+  if (nfull < nblk) block(nfull, std::true_type());
 
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -203,7 +229,7 @@ __global__ void __launch_bounds__(kAwThreads, 1) attn_fwd_wg_kernel(const __grid
 #pragma unroll
     for (int kb = 0; kb < KB; ++kb)
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
+      for (int q = 0; q < NV / 8; ++q) {
         const int col = kb * 64 + 8 * q + 2 * (lane & 3);
         if (col < p.D)
           *reinterpret_cast<uint32_t*>(orow + col) =
@@ -244,7 +270,7 @@ struct alignas(64) AttnBwdParams {
 
 // P and dS of one 64-column block, in place: s becomes P, dp becomes dS (fp32).  KV: row = key (valid
 // per row), the column statistics lc / dc were loaded for this block; dQ: column = key, MASK when the
-// block's keys from kcol on may lie past Skv.
+// block's keys from kcol on may lie past Skv.  c S - L is one FFMA, as the expression always compiled to.
 template <bool KV, bool MASK>
 __device__ __forceinline__ void bwd_elementwise(float (&s)[32], float (&dp)[32], const float (&lc)[16],
                                                 const float (&dc)[16], const float (&lrow)[2],
@@ -266,7 +292,7 @@ __device__ __forceinline__ void bwd_elementwise(float (&s)[32], float (&dp)[32],
         d = drow[r];
         ok = !MASK || kcol + 8 * (i >> 2) + e < Skv;
       }
-      const float pv = ok ? exp2f(s[i + e] * c - l) : 0.f;
+      const float pv = ok ? exp2_ftz(__fmaf_rn(s[i + e], c, -l)) : 0.f;
       s[i + e] = pv;
       dp[i + e] = pv * (dp[i + e] - d);
     }
@@ -489,6 +515,19 @@ int encode_seq_map(CUtensorMap* m, const void* base, int HD, int S, int B, long 
   return encode_tmap(m, base, 3, dims, strides, box, estr);
 }
 
+template <int KB, int NV>
+cudaError_t launch_fwd(dim3 grid, cudaStream_t stream, const AttnWgParams& p) {
+  const size_t smem = KB * (2 + 2 * kAwStages) * kTile + 1024;
+  static bool attr = false;
+  if (!attr) {
+    const cudaError_t e = cudaFuncSetAttribute(attn_fwd_wg_kernel<KB, NV>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               static_cast<int>(smem));
+    if (e != cudaSuccess) return e;
+    attr = true;
+  }
+  return launch_pdl(attn_fwd_wg_kernel<KB, NV>, grid, dim3(kAwThreads), smem, stream, p);
+}
+
 template <bool KV, int NV>
 cudaError_t launch_bwd(dim3 grid, cudaStream_t stream, const AttnBwdParams& p) {
   const size_t smem = (4 + 2 * kBwdStages) * kTile + 1024;
@@ -520,25 +559,12 @@ int attn_fwd_wg(const void* q, const void* k, const void* v, void* out, float* l
   p.H = H; p.Sq = Sq; p.Skv = Skv; p.D = D; p.ldo = ldo;
   p.c = scale * 1.4426950408889634f;
   const dim3 grid((Sq + 127) / 128, H, B);
-  if (D <= 64) {
-    const size_t smem = (2 + 2 * kAwStages) * kTile + 1024;
-    static bool attr = false;
-    if (!attr) {
-      CUDA_TRY(cudaFuncSetAttribute(attn_fwd_wg_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    static_cast<int>(smem)));
-      attr = true;
-    }
-    CUDA_TRY(launch_pdl(attn_fwd_wg_kernel<1>, grid, dim3(kAwThreads), smem, stream, p));
-  } else {
-    const size_t smem = 2 * (2 + 2 * kAwStages) * kTile + 1024;
-    static bool attr = false;
-    if (!attr) {
-      CUDA_TRY(cudaFuncSetAttribute(attn_fwd_wg_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    static_cast<int>(smem)));
-      attr = true;
-    }
-    CUDA_TRY(launch_pdl(attn_fwd_wg_kernel<2>, grid, dim3(kAwThreads), smem, stream, p));
-  }
+  if (D <= 40)
+    CUDA_TRY((launch_fwd<1, 40>)(grid, stream, p));
+  else if (D <= 64)
+    CUDA_TRY((launch_fwd<1, 64>)(grid, stream, p));
+  else
+    CUDA_TRY((launch_fwd<2, 64>)(grid, stream, p));
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -214,6 +214,14 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// 2^x as one MUFU.EX2, results below 2^-126 flushed to zero.  exp2f (no fast-math) is ex2.approx.f32,
+// which ptxas wraps in a compare and two multiplies per call to produce denormal results; for
+// x >= -126 both return the same value.
+__device__ __forceinline__ float exp2_ftz(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
 // sigmoid via ex2.approx + rcp.approx (2 MUFU ops, ~2 ulp): an IEEE division costs ~8 more issue
 // slots per element, which is what bounds the GroupNorm / SiLU kernels (ncu: FMA / ALU pipes, not DRAM)
 __device__ __forceinline__ float frcp_approx(float d) {
