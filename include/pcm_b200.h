@@ -41,7 +41,11 @@ typedef struct {
 } pcm_bsrc;
 
 /* One K-program entry: nchunks consecutive 64-wide K blocks read from a[a_src] at channel a_c0..,
- * spatially shifted by (dw, dh) (zero filled outside the image), against b[b_src] columns b_k0... */
+ * spatially shifted by (dw, dh) (zero filled outside the image), against b[b_src] columns b_k0...
+ * Chunk c multiplies only the K columns both operands have, min(64, a.C - (a_c0 + 64c), b.K - (b_k0 + 64c))
+ * rounded up to 16 (TMA zero-fills the operand that ends first): a LoRA entry of rank r (8 <= r <= 256,
+ * r % 8 == 0) is ceil(r/64) chunks whose last one is r % 64 wide.  b_k0: a multiple of 64 for a K-blocked
+ * B source, of 8 otherwise. */
 typedef struct {
   int32_t a_src, b_src, dw, dh, nchunks, a_c0, b_k0;
   uint16_t n_lo, n_hi; /* n_hi > 0: the entry only contributes to output columns [n_lo, n_hi)
@@ -85,12 +89,15 @@ typedef struct {
                             launches. */
 } pcm_gemm_desc;
 
-/* LoRA weight-gradient descriptor: out[ch, r] += alpha * sum_m P[m(+tap), ch] * Q[m, r], r < 64.
+/* LoRA weight-gradient descriptor: out[ch, r] += alpha * sum_m P[m(+tap), ch] * Q[m, q_c0 + r] for the rank
+ * slice r < w = min(64, q.C - q_c0) (a positive multiple of 8); only those w columns of out are stored.  A
+ * rank r > 64 takes ceil(r/64) launches (q_c0 + 64j, out advanced by 64j ranks); a slice of a stacked Q
+ * narrower than 64 passes a q that ends at the layer's last rank column.
  * Replaces autograd's wgrad of the peft lora_A / lora_B modules (T15:1296). */
 typedef struct {
   pcm_asrc p;          /* [tokens, Cp] activation (or grad) */
-  pcm_asrc q;          /* [tokens, >=64] rank-side operand */
-  int32_t q_c0;        /* first column of the 64-wide slice of q */
+  pcm_asrc q;          /* [tokens, >= q_c0 + 8] rank-side operand */
+  int32_t q_c0;        /* first column of the (at most 64-wide) rank slice of q */
   int32_t lin;
   int32_t M;           /* tokens */
   int32_t geoW, geoH;
@@ -225,7 +232,8 @@ int pcm_adamw_clip(float* p, float* g, float* m, float* v, int64_t n, float* sta
  * reference loop; offered as the opt-in EMA target): targ = rate*targ + (1-rate)*src */
 int pcm_ema_update(float* targ, const float* src, int64_t n, float rate, void* stream);
 /* table: num_entries x 9 int64 {a_off, b_off, a_fwd, sb_fwd, sb_t, a_t, cin|taps<<32, n|r<<32,
- * work_begin}; writes bf16 operand copies A, s*B, (s*B)^T, A^T */
+ * work_begin}; writes bf16 operand copies A, s*B, (s*B)^T, A^T.  Work = min(r, 64) x 64 tiles: per entry
+ * ceil(r/64) * (taps*cin/64 + n/64), work_begin its prefix sum, total_work the sum */
 int pcm_lora_refresh(const float* master, const void* table, int num_entries, int64_t total_work,
                      float scale, void* opnd, void* stream);
 

@@ -55,6 +55,17 @@ class UNetConfig:
         return self.lora_alpha / self.lora_rank
 
 
+LORA_RANKS = "8 <= r <= 256 with r % 8 == 0"
+
+
+def check_lora_rank(r):
+    """Raise ValueError unless r is a supported LoRA rank: 8 <= r <= 256, r % 8 == 0 (a [M, r] bf16 row of
+    the rank-side operands must be a multiple of 16 bytes for TMA)."""
+    if isinstance(r, bool) or not isinstance(r, int) or not (8 <= r <= 256 and r % 8 == 0):
+        raise ValueError(f"unsupported LoRA rank {r!r}: the supported ranks are {LORA_RANKS}")
+    return r
+
+
 SD15 = UNetConfig()
 # small configuration for fast parity tests (same topology, narrower)
 TINY = UNetConfig(block_out_channels=(64, 128, 128, 128), cross_attention_dim=64, num_heads=2)

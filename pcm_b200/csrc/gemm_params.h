@@ -11,6 +11,9 @@ struct KEntry {
   unsigned short n_lo, n_hi;  // n_hi > 0: entry applies to tiles with n_lo <= n0 < n_hi only
   int m_hi;                   // > 0: entry applies to tiles with m0 < m_hi only (its A source has
                               // fewer rows than the output: LoRA T of the leading samples)
+  int kend;                   // K columns both operands have from the entry's start:
+                              // min(a.C - a_c0, b.K - b_k0); chunk c multiplies min(64, kend - 64c)
+                              // of them, rounded up to 16 (narrow kernels only)
 };
 
 struct alignas(64) GemmParams {

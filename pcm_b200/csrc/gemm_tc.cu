@@ -4,8 +4,9 @@
 //               +residual, optional SiLU).  A is gathered by TMA from up to 6 NHWC bf16 tensors
 //               through a "K program" (spatial taps x channel chunks x K segments), so the same
 //               kernel runs nn.Linear, 1x1 / 3x3 / stride-2 convolutions (parity planes),
-//               skip-concat convolutions (two K segments), the LoRA up-projection fused as an
-//               extra 64-wide K segment, and all of their dgrads (taps mirrored, W transposed).
+//               skip-concat convolutions (two K segments), the LoRA up-projection fused as
+//               ceil(r/64) extra K chunks (a chunk only as wide as both operands: NARROW kernels),
+//               and all of their dgrads (taps mirrored, W transposed).
 //   pcm_wgrad : out[ch, r] += alpha * sum_m P[m(+tap), ch] * Q[m, r]   (LoRA A/B weight grads),
 //               both operands MN-major straight from the activation layout, split over tokens.
 //
@@ -47,7 +48,17 @@ __device__ __forceinline__ int tile_kblocks(const GemmParams& p, int m0, int n0)
   return nkb;
 }
 
-template <int BN>
+// k16 steps of chunk c of an entry whose operands share kend K columns: the chunk's width rounded up
+// to 16 (TMA zero-fills the operand that ends first, so the skipped products are exact zeros)
+__device__ __forceinline__ int chunk_ksteps(int kend, int c) {
+  const int w = kend - 64 * c;
+  return w >= 64 ? 4 : (w <= 16 ? 1 : (w + 15) >> 4);
+}
+
+// NARROW: some K chunk of the program is narrower than 64 (a LoRA rank r % 64 != 0); the producer
+// publishes each stage's k16 step count and the consumers issue only those.  Launches without a
+// narrow chunk run the plain 4-step mainloop.
+template <int BN, bool NARROW>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -55,6 +66,7 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
                                              ~static_cast<uintptr_t>(1023));
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
+  __shared__ int stage_ksteps[NARROW ? kMaxStages : 1];
 
   const int wg = threadIdx.x >> 7;
   const int S = p.num_stages;
@@ -114,6 +126,8 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
           for (int c = 0; c < en.nchunks; ++c, ++kidx) {
             if (kidx < kb0 || kidx >= kb1) continue;
             mbar_wait(&empty_bar[stage], phase ^ 1);
+            // (the arrive releases this store to the consumers' wait on the full barrier)
+            if constexpr (NARROW) stage_ksteps[stage] = chunk_ksteps(en.kend, c);
             mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
             uint8_t* sa = smem + stage * stage_bytes;
             uint8_t* sb = sa + kATileBytes;
@@ -161,10 +175,19 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
         const uint32_t a_addr = smem_u32(smem + stage * stage_bytes) + cw * (64 * 128);
         const uint32_t b_addr = smem_u32(smem + stage * stage_bytes) + kATileBytes;
         wgmma_fence();
+        if constexpr (NARROW) {
+          const int nk = stage_ksteps[stage];   // warpgroup-uniform
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          Wgmma<BN, 0, 0>::mma(acc, wgmma_desc_sw128(a_addr + k * 32, 16, 1024),
-                               wgmma_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
+          for (int k = 0; k < 4; ++k)
+            if (k < nk)
+              Wgmma<BN, 0, 0>::mma(acc, wgmma_desc_sw128(a_addr + k * 32, 16, 1024),
+                                   wgmma_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
+        } else {
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            Wgmma<BN, 0, 0>::mma(acc, wgmma_desc_sw128(a_addr + k * 32, 16, 1024),
+                                 wgmma_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
+        }
         wgmma_commit();
         wgmma_fence_acc(acc);
         // the previous K block's wgmma are complete: its stage may be refilled
@@ -249,6 +272,7 @@ struct alignas(64) WgradParams {
   CUtensorMap q_map;
   int lin, geoW, geoHW;
   int M, Cp, q_c0;
+  int qw;    // rank columns of the slice: min(64, q.C - q_c0); stores are masked to them
   int num_taps;
   int dw[9], dh[9];
   long long tap_off[9];
@@ -378,6 +402,7 @@ pcm_wgrad_kernel(const __grid_constant__ WgradParams p) {
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
           const int r = 8 * q + fcol;
+          if (r >= p.qw) break;   // past the slice's ranks (qw is a multiple of 8: r + 1 < qw too)
           const float v0 = acc[4 * q + 2 * h] * p.alpha, v1 = acc[4 * q + 2 * h + 1] * p.alpha;
           if (p.os_col == 1) {   // rank index contiguous (dB layout [n][r]): 8-byte vector reductions
             asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(o + r), "f"(v0), "f"(v1) : "memory");
@@ -429,16 +454,17 @@ static int encode_asrc(CUtensorMap* map, const pcm_asrc& a, int lin, int geoW, i
 
 // the wgmma N of the kernel is the N tile of the launch
 typedef void (*GemmKernel)(const GemmParams);
+template <bool NARROW>
 static GemmKernel gemm_kernel_for(int block_n) {
   switch (block_n) {
-    case 32: return pcm_gemm_kernel<32>;
-    case 64: return pcm_gemm_kernel<64>;
-    case 96: return pcm_gemm_kernel<96>;
-    case 128: return pcm_gemm_kernel<128>;
-    case 160: return pcm_gemm_kernel<160>;
-    case 192: return pcm_gemm_kernel<192>;
-    case 224: return pcm_gemm_kernel<224>;
-    default: return pcm_gemm_kernel<256>;
+    case 32: return pcm_gemm_kernel<32, NARROW>;
+    case 64: return pcm_gemm_kernel<64, NARROW>;
+    case 96: return pcm_gemm_kernel<96, NARROW>;
+    case 128: return pcm_gemm_kernel<128, NARROW>;
+    case 160: return pcm_gemm_kernel<160, NARROW>;
+    case 192: return pcm_gemm_kernel<192, NARROW>;
+    case 224: return pcm_gemm_kernel<224, NARROW>;
+    default: return pcm_gemm_kernel<256, NARROW>;
   }
 }
 
@@ -473,12 +499,18 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
     }
   }
   int nkb = 0;
+  bool narrow = false;
   for (int e = 0; e < d->num_prog; ++e) {
     const pcm_kentry& k = d->prog[e];
+    // K-blocked weights are addressed in whole 64-wide blocks; a row-major B only needs its K offset to
+    // start a 16-byte segment (TMA global addresses and strides are 16-byte multiples)
     if (k.a_src < 0 || k.a_src >= d->num_a || k.b_src < 0 || k.b_src >= d->num_b || k.nchunks < 1 ||
-        (k.b_k0 & 63) != 0)
+        k.a_c0 < 0 || k.b_k0 < 0 || (k.b_k0 & (d->b[k.b_src].kblocked ? 63 : 7)) != 0)
       return set_error("pcm_gemm: bad K program entry");
-    p.prog[e] = KEntry{k.a_src, k.b_src, k.dw, k.dh, k.nchunks, k.a_c0, k.b_k0, k.n_lo, k.n_hi, 0};
+    const int a_left = d->a[k.a_src].C - k.a_c0, b_left = d->b[k.b_src].K - k.b_k0;
+    const int kend = a_left < b_left ? a_left : b_left;
+    if (kend < 64 * k.nchunks) narrow = true;
+    p.prog[e] = KEntry{k.a_src, k.b_src, k.dw, k.dh, k.nchunks, k.a_c0, k.b_k0, k.n_lo, k.n_hi, 0, kend};
     {  // an A source with fewer rows than the output only feeds the leading M tiles (TMA would zero
        // fill the rest: skip those K blocks instead); whole tiles only
       const pcm_asrc& a = d->a[k.a_src];
@@ -534,11 +566,11 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
   }
 
   const size_t smem = static_cast<size_t>(S) * stage_bytes + kStagingBytes + 1024;
-  const GemmKernel kernel = gemm_kernel_for(d->block_n);
-  static bool attr_set[9] = {};
-  if (!attr_set[d->block_n / 32]) {
+  const GemmKernel kernel = narrow ? gemm_kernel_for<true>(d->block_n) : gemm_kernel_for<false>(d->block_n);
+  static bool attr_set[2][9] = {};
+  if (!attr_set[narrow][d->block_n / 32]) {
     CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-    attr_set[d->block_n / 32] = true;
+    attr_set[narrow][d->block_n / 32] = true;
   }
   if (d->dep_a_src1 > 0 && p.ksplit == 1) {  // (split-K: the finalize kernel follows; keep the plain chain)
     if (d->dep_a_src1 > d->num_a) return set_error("pcm_gemm: bad dep_a_src1");
@@ -578,6 +610,9 @@ static int launch_wgrad(const pcm_wgrad_desc* d, cudaStream_t stream) {
   p.M = d->M;
   p.Cp = d->p.C;
   p.q_c0 = d->q_c0;
+  p.qw = d->q.C - d->q_c0 < 64 ? d->q.C - d->q_c0 : 64;
+  if (d->q_c0 < 0 || p.qw < 8 || p.qw % 8 != 0)
+    return set_error("pcm_wgrad: the rank slice q[:, q_c0:] must hold a positive multiple of 8 columns");
   p.num_taps = d->num_taps;
   for (int t = 0; t < d->num_taps; ++t) {
     p.dw[t] = d->dw[t];

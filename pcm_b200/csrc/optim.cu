@@ -104,10 +104,12 @@ struct RefreshEntry {
   long long work_begin;                // prefix sum of per-entry 64x64 tiles (A tiles, then B tiles)
 };
 
-// One block per 64x64 fp32 tile (r = 64): coalesced read, bf16 copy in the source layout, and the
-// transposed copy through shared memory so both writes are 128-byte contiguous per row.
-//   A tile (rows r, columns [c0, c0+64) of tap t): a_fwd[r][t*cin + c]  and  a_t[c][t*64 + r]
-//   B tile (rows n0.., columns r):                 sb_fwd[n][r] = s*B   and  sb_t[r][n]
+// One block per (rank tile, 64-column tile): rank tile j holds ranks [64j, 64j + rh), rh = min(64, r - 64j),
+// so r <= 64 is one tile of r rows and r > 64 is split into 64-row tiles.  Coalesced read, bf16 copy in
+// the source layout, and the transposed copy through shared memory so both writes are contiguous rows.
+//   A tile (ranks, columns [c0, c0+64) of tap t): a_fwd[r][t*cin + c]  and  a_t[c][t*r + r]
+//   B tile (rows n0.., ranks):                    sb_fwd[n][r] = s*B   and  sb_t[r][n]
+// Per entry: ceil(r/64) * (taps*cin/64) A tiles, then ceil(r/64) * (n/64) B tiles (r % 8 == 0).
 __global__ void __launch_bounds__(256) lora_refresh_kernel(const float* __restrict__ master,
                                                            const RefreshEntry* __restrict__ tab,
                                                            int num_entries, float scale,
@@ -128,52 +130,65 @@ __global__ void __launch_bounds__(256) lora_refresh_kernel(const float* __restri
   }
   __syncthreads();
   const int ktot = e.taps * e.cin;
-  const long long a_tiles = ktot / 64;
-  const bool is_a = tidx < a_tiles;
+  const int rtiles = (e.r + 63) / 64;
+  const long long a_cols = ktot / 64;
+  const bool is_a = tidx < rtiles * a_cols;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;  // 16 float4 columns x 16 rows
   if (is_a) {
-    const int c0 = static_cast<int>(tidx) * 64;  // column in [0, taps*cin); one tap per tile
+    const int j = static_cast<int>(tidx / a_cols);
+    const int c0 = static_cast<int>(tidx - j * a_cols) * 64;  // column in [0, taps*cin); one tap per tile
+    const int r0 = 64 * j, rh = min(64, e.r - r0);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int r = ty + 16 * i;
-      const float4 v = *reinterpret_cast<const float4*>(master + e.a_off + static_cast<long long>(r) * ktot + c0 + tx * 4);
+      if (r >= rh) break;
+      const float4 v = *reinterpret_cast<const float4*>(master + e.a_off + static_cast<long long>(r0 + r) * ktot + c0 + tx * 4);
       tile[r][tx * 4] = v.x; tile[r][tx * 4 + 1] = v.y; tile[r][tx * 4 + 2] = v.z; tile[r][tx * 4 + 3] = v.w;
       uint2 u;
       u.x = pack_bf16x2(v.x, v.y);
       u.y = pack_bf16x2(v.z, v.w);
-      *reinterpret_cast<uint2*>(opnd + e.a_fwd + static_cast<long long>(r) * ktot + c0 + tx * 4) = u;
+      *reinterpret_cast<uint2*>(opnd + e.a_fwd + static_cast<long long>(r0 + r) * ktot + c0 + tx * 4) = u;
     }
     __syncthreads();
     const int t = c0 / e.cin, cc0 = c0 - t * e.cin;
+    if (tx * 4 < rh) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int c = ty + 16 * i;  // a_t row (input channel), 64 consecutive r
-      uint2 u;
-      u.x = pack_bf16x2(tile[tx * 4][c], tile[tx * 4 + 1][c]);
-      u.y = pack_bf16x2(tile[tx * 4 + 2][c], tile[tx * 4 + 3][c]);
-      *reinterpret_cast<uint2*>(opnd + e.a_t + (static_cast<long long>(cc0 + c) * e.taps + t) * 64 + tx * 4) = u;
+      for (int i = 0; i < 4; ++i) {
+        const int c = ty + 16 * i;  // a_t row (input channel), 4 consecutive ranks per thread
+        uint2 u;
+        u.x = pack_bf16x2(tile[tx * 4][c], tile[tx * 4 + 1][c]);
+        u.y = pack_bf16x2(tile[tx * 4 + 2][c], tile[tx * 4 + 3][c]);
+        *reinterpret_cast<uint2*>(opnd + e.a_t + (static_cast<long long>(cc0 + c) * e.taps + t) * e.r + r0 + tx * 4) = u;
+      }
     }
   } else {
-    const int n0 = static_cast<int>(tidx - a_tiles) * 64;
+    const long long bt = tidx - rtiles * a_cols;
+    const long long n_tiles = e.n / 64;
+    const int j = static_cast<int>(bt / n_tiles);
+    const int n0 = static_cast<int>(bt - j * n_tiles) * 64;
+    const int r0 = 64 * j, rh = min(64, e.r - r0);
+    if (tx * 4 < rh) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int nn = ty + 16 * i;
-      float4 v = *reinterpret_cast<const float4*>(master + e.b_off + static_cast<long long>(n0 + nn) * 64 + tx * 4);
-      v.x *= scale; v.y *= scale; v.z *= scale; v.w *= scale;
-      tile[nn][tx * 4] = v.x; tile[nn][tx * 4 + 1] = v.y; tile[nn][tx * 4 + 2] = v.z; tile[nn][tx * 4 + 3] = v.w;
-      uint2 u;
-      u.x = pack_bf16x2(v.x, v.y);
-      u.y = pack_bf16x2(v.z, v.w);
-      *reinterpret_cast<uint2*>(opnd + e.sb_fwd + static_cast<long long>(n0 + nn) * 64 + tx * 4) = u;
+      for (int i = 0; i < 4; ++i) {
+        const int nn = ty + 16 * i;
+        float4 v = *reinterpret_cast<const float4*>(master + e.b_off + static_cast<long long>(n0 + nn) * e.r + r0 + tx * 4);
+        v.x *= scale; v.y *= scale; v.z *= scale; v.w *= scale;
+        tile[nn][tx * 4] = v.x; tile[nn][tx * 4 + 1] = v.y; tile[nn][tx * 4 + 2] = v.z; tile[nn][tx * 4 + 3] = v.w;
+        uint2 u;
+        u.x = pack_bf16x2(v.x, v.y);
+        u.y = pack_bf16x2(v.z, v.w);
+        *reinterpret_cast<uint2*>(opnd + e.sb_fwd + static_cast<long long>(n0 + nn) * e.r + r0 + tx * 4) = u;
+      }
     }
     __syncthreads();
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int r = ty + 16 * i;  // sb_t row, 64 consecutive n
+      if (r >= rh) break;
       uint2 u;
       u.x = pack_bf16x2(tile[tx * 4][r], tile[tx * 4 + 1][r]);
       u.y = pack_bf16x2(tile[tx * 4 + 2][r], tile[tx * 4 + 3][r]);
-      *reinterpret_cast<uint2*>(opnd + e.sb_t + static_cast<long long>(r) * e.n + n0 + tx * 4) = u;
+      *reinterpret_cast<uint2*>(opnd + e.sb_t + static_cast<long long>(r0 + r) * e.n + n0 + tx * 4) = u;
     }
   }
 }
@@ -219,7 +234,8 @@ extern "C" int pcm_ema_update(float* targ, const float* src, int64_t n, float ra
 
 extern "C" int pcm_lora_refresh(const float* master, const void* table, int num_entries,
                                 int64_t total_work, float scale, void* opnd, void* stream) {
-  // total_work = number of 64x64 tiles (r must be 64; cin and n multiples of 64)
+  // total_work = number of tiles: per entry ceil(r/64) * (taps*cin/64 + n/64) (r % 8 == 0; cin and n
+  // multiples of 64)
   CUDA_TRY(launch_pdl(lora_refresh_kernel, dim3(static_cast<unsigned>(total_work)), dim3(256), 0, ST(stream), master, reinterpret_cast<const RefreshEntry*>(table), num_entries, scale,
       reinterpret_cast<bf16*>(opnd)));
   CUDA_TRY(cudaGetLastError());

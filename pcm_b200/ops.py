@@ -33,6 +33,11 @@ def asrc_mat(t):
     return L.ASrc(t.data_ptr(), Cc, M, 1, 1, t.stride(0), t.stride(0) * M, t.stride(0) * M)
 
 
+def asrc_cols(a, C):
+    """The same A source seen with only its first C channels (TMA zero-fills past them)."""
+    return L.ASrc(a.ptr, C, a.W, a.H, a.B, a.sW, a.sH, a.sB)
+
+
 def kblock(w):
     """[N, K] row-major -> K-blocked [K/64, N, 64] (see pcm_bsrc.kblocked): the frozen weights are
     stored this way so that the N x 64 operand tile of a K block is contiguous in HBM."""
@@ -98,15 +103,25 @@ def pick_tiling(M, N, nkb):
     return pick_block_n(M, N), 1
 
 
-def gemm_flops(a_srcs, prog, M, N, lin, geo):
-    """ALGORITHMIC flops of one launch: an N-ranged K entry only counts its own output columns and an A
-    source with fewer rows than the output (the LoRA T of the leading samples) only its own rows."""
+def chunk_widths(a_srcs, b_srcs, e):
+    """K columns each 64-wide chunk of K-program entry e multiplies: those both operands have,
+    min(64, a.C - (a_c0 + 64c), b.K - (b_k0 + 64c)) (a LoRA rank r % 64 != 0 ends the last chunk early;
+    the kernel rounds the width up to 16, multiplying TMA-filled zeros)."""
+    kend = min(a_srcs[e[0]].C - e[5], b_srcs[e[1]].K - e[6])
+    return [max(0, min(64, kend - 64 * c)) for c in range(e[4])]
+
+
+def gemm_flops(a_srcs, prog, M, N, lin, geo, b_srcs=None):
+    """ALGORITHMIC flops of one launch: an N-ranged K entry only counts its own output columns, an A
+    source with fewer rows than the output (the LoRA T of the leading samples) only its own rows, and a
+    chunk only the K columns both operands have (with b_srcs)."""
     fl = 0.0
     for e in prog:
         a = a_srcs[e[0]]
         rows = min(M, a.W if lin else a.B * geo[0] * geo[1])
         cols = min(N, e[8] - e[7]) if (len(e) > 7 and e[8]) else N
-        fl += 2.0 * rows * cols * 64 * e[4]
+        k = 64 * e[4] if b_srcs is None else sum(chunk_widths(a_srcs, b_srcs, e))
+        fl += 2.0 * rows * cols * k
     return fl
 
 
@@ -179,7 +194,7 @@ def gemm(a_srcs, b_srcs, prog, *, lin, M, N, out, geo=(1, 1), bias=None, rowvec=
                                      prog=[tuple(e) for e in prog], num_a=len(a_srcs), num_b=len(b_srcs),
                                      a_C=[a.C for a in a_srcs], b_K=[b.K for b in b_srcs],
                                      b_N=[b.N for b in b_srcs], dep=dep_a_src,
-                                     flop=gemm_flops(a_srcs, prog, M, N, lin, geo))))
+                                     flop=gemm_flops(a_srcs, prog, M, N, lin, geo, b_srcs))))
         return out
     if PROFILE is not None:
         e0 = torch.cuda.Event(enable_timing=True, external=PROFILE_EXTERNAL)
@@ -187,7 +202,7 @@ def gemm(a_srcs, b_srcs, prog, *, lin, M, N, out, geo=(1, 1), bias=None, rowvec=
         e0.record()
         L.check(L.lib().pcm_gemm(C.byref(d), _stream()), "pcm_gemm")
         e1.record()
-        PROFILE.append((e0, e1, gemm_flops(a_srcs, prog, M, N, lin, geo)))
+        PROFILE.append((e0, e1, gemm_flops(a_srcs, prog, M, N, lin, geo, b_srcs)))
         return out
     L.check(L.lib().pcm_gemm(C.byref(d), _stream()), "pcm_gemm")
     return out

@@ -119,6 +119,7 @@ def parse_args(argv=None, extra=None):
         # GradScaler / overflow skipping needed) - documented deviation, DESIGN.md section 4.
         print("pcm_b200: --mixed_precision fp16 runs the bf16 path (same rate, wider range, no loss scaling)",
               file=sys.stderr)
+    config.check_lora_rank(args.lora_rank)        # peft takes any r; the kernels take 8 <= r <= 256, r % 8 == 0
     if args.lr_scheduler not in lr_schedules.SCHEDULES:
         raise ValueError(f"{args.lr_scheduler} is not a valid SchedulerType, please select one of "
                          f"{list(lr_schedules.SCHEDULES)}.")
@@ -158,7 +159,7 @@ def save_state(st, cfg, path, global_step, gen):
     """accelerator.save_state (T15:1339-1341): adapter weights + optimiser state + RNG."""
     save_lora(st, cfg, path)
     sd = st.state_dict()
-    sd.update(global_step=global_step, rng_state=gen.get_state())
+    sd.update(global_step=global_step, rng_state=gen.get_state(), lora_rank=cfg.lora_rank)
     torch.save(sd, os.path.join(path, "pcm_b200_state.pt"))
 
 
@@ -168,6 +169,9 @@ def load_state(st, path, gen):
     if not os.path.exists(f):
         raise FileNotFoundError(f"{f} not found: checkpoints written before optimiser state was saved cannot be resumed")
     sd = torch.load(f)
+    if sd.get("lora_rank", st.unet.r) != st.unet.r:
+        raise ValueError(f"{path} holds a rank-{sd['lora_rank']} LoRA adapter; this run trains rank {st.unet.r} "
+                         f"(--lora_rank must match the checkpoint to resume from it)")
     st.load_state_dict(sd)
     gen.set_state(sd["rng_state"])
     return int(sd["global_step"])

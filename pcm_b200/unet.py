@@ -5,8 +5,9 @@ Mirrors the call `unet(sample, timestep, encoder_hidden_states=...).sample` of d
 UNet2DConditionModel wrapped by peft (train_pcm_lora_sd15.py:1192-1198 student, :1219-1244
 teacher, :1263-1268 target) and its autograd backward (:1296), with:
   * activations NHWC bf16, one rounding per materialised tensor (bf16 autocast semantics);
-  * LoRA unmerged: T = A(x) as a 64-wide GEMM, then s*B*T enters the base GEMM as one extra
-    64-wide K block (same wgmma accumulator), so `base(x) + B(A(x)) * scaling` is one kernel;
+  * LoRA unmerged (rank 8 <= r <= 256, r % 8 == 0): T = A(x) as an r-wide GEMM, then s*B*T enters the
+    base GEMM as ceil(r/64) extra K blocks, the last one r % 64 wide (same wgmma accumulator), so
+    `base(x) + B(A(x)) * scaling` is one kernel;
   * skip concats never materialised (two K segments / two GroupNorm sources);
   * backward = explicit tape: dgrad through every layer, wgrad for LoRA factors only.
 Parameters use diffusers state-dict names; LoRA factors live in ONE flat fp32 buffer
@@ -21,7 +22,7 @@ from typing import Optional
 import torch
 
 from . import ops
-from .config import UNetConfig, is_lora_target, layer_table
+from .config import UNetConfig, check_lora_rank, is_lora_target, layer_table
 
 BF16 = torch.bfloat16
 TAPS3 = ops.TAPS3
@@ -114,7 +115,8 @@ class UNetB200:
         inputs; backward() runs each block's forward again right before its backward (see forward())."""
         self.cfg, self.dev = cfg, device
         self.gradient_checkpointing = gradient_checkpointing
-        self.r = cfg.lora_rank
+        self.r = check_lora_rank(cfg.lora_rank) if lora else cfg.lora_rank
+        self.rc = (self.r + 63) // 64       # 64-wide K chunks / weight-gradient rank slices of one adapter
         self.scale = cfg.lora_scale
         self.layers = {}
         self.has_lora = lora
@@ -163,6 +165,9 @@ class UNetB200:
                 taps = k * k if kind == "conv" else 1
                 A = state_dict[name + ".lora_A.weight"].float()
                 Bm = state_dict[name + ".lora_B.weight"].float()
+                if A.shape[0] != self.r or Bm.shape[1] != self.r:
+                    raise ValueError(f"{name}: the state dict holds a rank-{A.shape[0]} LoRA adapter "
+                                     f"(lora_B rank {Bm.shape[1]}), the UNet is configured for rank {self.r}")
                 if kind == "conv":
                     A = A.permute(0, 2, 3, 1)
                 A = A.reshape(self.r, taps * cin)
@@ -214,8 +219,9 @@ class UNetB200:
                 lo.gB = self.lora_grad[lo.b_off:lo.b_off + nb].view(L.cout, self.r)
                 rows.append([lo.a_off, lo.b_off, a_fwd, sb_fwd, sb_t, a_t, L.cin | (taps << 32),
                              L.cout | (self.r << 32), work])
-                assert self.r == 64 and L.cin % 64 == 0 and L.cout % 64 == 0
-                work += (taps * L.cin) // 64 + L.cout // 64     # 64x64 tiles of A, then of B
+                assert L.cin % 64 == 0 and L.cout % 64 == 0
+                # (min(r, 64) x 64) tiles of A, then of B, per 64-rank slice
+                work += self.rc * ((taps * L.cin) // 64 + L.cout // 64)
             self.refresh_table = torch.tensor(rows, dtype=torch.int64, device=device)
             self.refresh_work = work
             self.refresh_lora()
@@ -333,7 +339,7 @@ class UNetB200:
         if T is not None:
             srcs.append(ops.asrc_mat(T))
             bs.append(ops.bsrc(sb_stack))
-            prog += [(1, 1, 0, 0, 1, t_c0, 0, n_lo, n_hi) for t_c0, n_lo, n_hi in ranges]
+            prog += [(1, 1, 0, 0, self.rc, t_c0, 0, n_lo, n_hi) for t_c0, n_lo, n_hi in ranges]
         out = self._new(x.shape[0], N)
         ops.gemm(srcs, bs, prog, lin=True, M=x.shape[0], N=N, out=out, bias=bias, block_n=block_n,
                  dep_a_src=dep_a_src)
@@ -571,7 +577,7 @@ class UNetB200:
             srcs_l, prog_l = (srcs, prog) if lbn == B else self._conv_prog(xl, 3, stride, L.cin)
             ops.gemm(srcs_l, [ops.bsrc(L.lora.a_fwd)], prog_l, lin=False, M=lbn * Ho * Wo, N=self.r,
                      geo=(Wo, Ho), out=T.view(lbn * Ho * Wo, self.r))
-            prog = prog + [(len(srcs), 1, 0, 0, 1, 0, 0)]
+            prog = prog + [(len(srcs), 1, 0, 0, self.rc, 0, 0)]
             srcs = srcs + [ops.asrc_nhwc(T)]
             bs.append(ops.bsrc(L.lora.sb_fwd))
         out = self._new(B, Ho, Wo, N, dtype=torch.float32 if out_fp32 else BF16)
@@ -601,7 +607,7 @@ class UNetB200:
             T = self._new(Ml, self.r)
             srcs_l = srcs if Ml == M else [ops.asrc_mat(x) for x in xl]
             ops.gemm(srcs_l, [ops.bsrc(L.lora.a_fwd)], prog, lin=True, M=Ml, N=self.r, out=T)
-            prog = prog + [(len(srcs), 1, 0, 0, 1, 0, 0)]
+            prog = prog + [(len(srcs), 1, 0, 0, self.rc, 0, 0)]
             srcs = srcs + [ops.asrc_mat(T)]   # Ml rows: tiles past them read zeros (TMA bounds)
             bs.append(ops.bsrc(L.lora.sb_fwd))
         out = self._new(M, N)
@@ -913,11 +919,19 @@ class UNetB200:
         """LoRA weight gradients of layer L (called inside _Side): dB += s * dy^T T[:, t_c0:t_c0+r] and
         dA += dt[:, dt_c0:dt_c0+r]^T x for each (x, taps, tap offsets) of P_list.  dy, T, dt: A-operand
         sources with M rows."""
-        lo = L.lora
-        ops.wgrad(dy, T, lo.gB, lin=True, M=M, os_row=self.r, os_col=1, alpha=self.scale, q_c0=t_c0)
-        for psrc, taps, offs in P_list:
-            ops.wgrad(psrc, dt, lo.gA, lin=lin, M=M, geo=geo, taps=taps, tap_off=offs, os_row=1,
-                      os_col=lo.gA.shape[1], q_c0=dt_c0)
+        lo, r = L.lora, self.r
+        if r % 64:
+            # the kernel's rank slice is min(64, q.C - q_c0) wide: end stacked T / dT views at this
+            # layer's last rank column so that no slice reaches into the next layer's columns
+            T, dt = ops.asrc_cols(T, t_c0 + r), ops.asrc_cols(dt, dt_c0 + r)
+        # one launch per 64-rank slice j (r > 64): ranks [64j, 64j + 64) of gB's rows / gA's rows
+        for j in range(self.rc):
+            ops.wgrad(dy, T, lo.gB[:, 64 * j:], lin=True, M=M, os_row=r, os_col=1, alpha=self.scale,
+                      q_c0=t_c0 + 64 * j)
+        for j in range(self.rc):
+            for psrc, taps, offs in P_list:
+                ops.wgrad(psrc, dt, lo.gA[64 * j:], lin=lin, M=M, geo=geo, taps=taps, tap_off=offs, os_row=1,
+                          os_col=lo.gA.shape[1], q_c0=dt_c0 + 64 * j)
 
     def linear_bwd(self, rec, dy, need_dx=True, t_c0=0):
         """rec: LinearRec (or TembRec, whose block of T starts at column t_c0).  Returns dx [M, cin_total]
@@ -944,7 +958,7 @@ class UNetB200:
         if dt is not None:
             srcs.append(ops.asrc_mat(dt))
             bs.append(ops.bsrc(L.lora.a_t))
-            prog.append((1, 1, 0, 0, 1, 0, 0))
+            prog.append((1, 1, 0, 0, self.rc, 0, 0))
         dx = self._new(M, L.cin)
         ops.gemm(srcs, bs, prog, lin=True, M=M, N=L.cin, out=dx, dep_a_src=None if dt is None else 1)
         return dx
@@ -959,9 +973,16 @@ class UNetB200:
         dT = None
         if T is not None:
             dT = self._new(M, g * r)
-            prog = [(0, 0, 0, 0, Cc // 64, i * Cc, 0, i * r, (i + 1) * r) for i in range(g)]
-            ops.gemm([ops.asrc_mat(dpk)], [ops.bsrc(G.sbt_stack)], prog, lin=True, M=M, N=g * r, out=dT,
-                     block_n=64)
+            if r % 32 == 0:
+                # one GEMM, layer i's K range feeding its own N range [i*r, (i+1)*r): block_n must divide r
+                prog = [(0, 0, 0, 0, Cc // 64, i * Cc, 0, i * r, (i + 1) * r) for i in range(g)]
+                ops.gemm([ops.asrc_mat(dpk)], [ops.bsrc(G.sbt_stack)], prog, lin=True, M=M, N=g * r, out=dT,
+                         block_n=64 if r % 64 == 0 else 32)
+            else:
+                # N ranges that no block_n can align to: one GEMM per layer into its columns of dT
+                for i in range(g):
+                    ops.gemm([ops.asrc_mat(dpk)], [ops.bsrc(G.sbt_stack[i * r:(i + 1) * r])],
+                             [(0, 0, 0, 0, Cc // 64, i * Cc, 0)], lin=True, M=M, N=r, out=dT[:, i * r:(i + 1) * r])
             with UNetB200._Side(self, (dpk, T, dT, x)):
                 for i, L in enumerate(G.layers):
                     self._lora_wgrads(L, M, ops.asrc_mat(dpk[:, i * Cc:(i + 1) * Cc]), ops.asrc_mat(T),
@@ -975,7 +996,7 @@ class UNetB200:
             srcs.append(ops.asrc_mat(dT))
             for i, L in enumerate(G.layers):
                 bs.append(ops.bsrc(L.lora.a_t))
-                prog.append((1, 1 + i, 0, 0, 1, i * r, 0))
+                prog.append((1, 1 + i, 0, 0, self.rc, i * r, 0))
         dx = self._new(M, G.cin)
         ops.gemm(srcs, bs, prog, lin=True, M=M, N=G.cin, out=dx, dep_a_src=None if dT is None else 1)
         return dx
@@ -1016,7 +1037,7 @@ class UNetB200:
             if dt is not None:
                 srcs.append(ops.asrc_nhwc(dt))
                 bs.append(ops.bsrc(L.lora.a_t))
-                prog += [(1, 1, -dw, -dh, 1, 0, t * self.r) for t, (dw, dh) in enumerate(TAPS3)]
+                prog += [(1, 1, -dw, -dh, self.rc, 0, t * self.r) for t, (dw, dh) in enumerate(TAPS3)]
             dx = self._new(B, Ho, Wo, cin)
             ops.gemm(srcs, bs, prog, lin=False, M=M, N=cin, geo=geo, out=dx.view(M, cin),
                      dep_a_src=None if dt is None else 1)
@@ -1033,7 +1054,7 @@ class UNetB200:
                 if dt is not None:
                     srcs.append(ops.asrc_nhwc(dt))
                     bs.append(ops.bsrc(L.lora.a_t))
-                    prog += [(1, 1, dw, dh, 1, 0, t * self.r) for t, dw, dh in taps]
+                    prog += [(1, 1, dw, dh, self.rc, 0, t * self.r) for t, dw, dh in taps]
                 plane = dx[:, p::2, q::2, :]
                 ops.gemm(srcs, bs, prog, lin=False, M=M, N=cin, geo=geo, out=plane,
                          out_strides=(plane.stride(2), plane.stride(1), plane.stride(0)), epi=(Wo, Wo * Ho),
