@@ -236,6 +236,22 @@ int pcm_ema_update(float* targ, const float* src, int64_t n, float rate, void* s
  * ceil(r/64) * (taps*cin/64 + n/64), work_begin its prefix sum, total_work the sum */
 int pcm_lora_refresh(const float* master, const void* table, int num_entries, int64_t total_work,
                      float scale, void* opnd, void* stream);
+/* LoRA fused into the frozen weights for inference (peft fuse_lora), out of place on the K-blocked
+ * [K/64][N_total][64] bf16 operands: dst[n0+n, k] = bf16(float(src[n0+n, k]) + scale * sum_r B[n,r] A[r,k]),
+ * fp32 sum in ascending rank order, one rounding.  table: num_entries x 8 int64 {a_off, b_off (fp32
+ * master elements; A [r][K], B [n][r]), src, dst (device addresses of the stacked operands),
+ * n0 | N_total<<32, K | r<<32, n, work_begin}; n and K multiples of 64, 8 <= r <= 256, r % 8 == 0.
+ * Work = 64 x 64 tiles: per entry (n/64) * (K/64), work_begin its prefix sum, total_work the sum */
+int pcm_lora_fuse(const float* master, const void* table, int num_entries, int64_t total_work, float scale,
+                  void* stream);
+/* One eta = 0 DDIM step of the few-step sampler (DDIMScheduler trailing, set_alpha_to_one=False) after
+ * the pipeline's CFG mix.  cfg != 0 (guidance scale > 1): eps holds 2B samples [uncond; cond] and is
+ * mixed eps_u + g (eps_c - eps_u) with g = *guidance (device double); cfg == 0: B samples, guidance unread.  pred_type 0 = epsilon, 1 = v_prediction.
+ * x_out = sqrt(a_prev) x0 + sqrt(1-a_prev) eps in double, rounded to fp32; x_out2 (may be NULL) gets the
+ * same values.  x_out may alias x. */
+int pcm_sample_step(const float* eps, const float* x, float* x_out, float* x_out2, int64_t per, int B,
+                    int cfg, const double* guidance, double sqrt_a_t, double sqrt_1m_a_t, double sqrt_a_prev,
+                    double sqrt_1m_a_prev, int pred_type, void* stream);
 
 #ifdef __cplusplus
 }

@@ -113,10 +113,12 @@ EXPORTS = [
     "pcm_adamw_clip",
     "pcm_ema_update",
     "pcm_lora_refresh",
+    "pcm_lora_fuse",
+    "pcm_sample_step",
 ]
 
 
-P, I, L64, F = C.c_void_p, C.c_int, C.c_int64, C.c_float
+P, I, L64, F, D = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
 ARGTYPES = {
     "pcm_gemm": [P, P],
     "pcm_wgrad": [P, P],
@@ -149,6 +151,8 @@ ARGTYPES = {
     "pcm_adamw_clip": [P, P, P, P, L64, P, F, F, F, F, F, F, P, I, P],
     "pcm_ema_update": [P, P, L64, F, P],
     "pcm_lora_refresh": [P, P, I, L64, F, P, P],
+    "pcm_lora_fuse": [P, P, I, L64, F, P],
+    "pcm_sample_step": [P, P, P, P, L64, I, I, P, D, D, D, D, I, P],
 }
 
 

@@ -375,6 +375,62 @@ __global__ void pcm_teacher_substep_kernel(const float* __restrict__ eps_c, cons
 }
 }  // namespace pcm
 
+// ------------------------------------------------------------------------------------------
+// One step of the few-step sampler (the reference's validation pipeline: StableDiffusionPipeline with
+// DDIMScheduler(timestep_spacing="trailing", set_alpha_to_one=False), eta = 0, T15:120-207):
+//   cfg:          eps = eps_u + g (eps_c - eps_u) on the [uncond; cond] batch of 2B samples, g = *guidance
+//                 (device memory, so one captured loop serves every guidance scale > 1)
+//   epsilon:      x0 = (x - sqrt(1-a_t) eps) / sqrt(a_t)
+//   v_prediction: x0 = sqrt(a_t) x - sqrt(1-a_t) v,  eps = sqrt(a_t) v + sqrt(1-a_t) x
+//   x_prev = sqrt(a_prev) x0 + sqrt(1-a_prev) eps
+// The four square roots are host doubles; the arithmetic runs in double with one rounding to fp32.
+// x_out2 (optional) receives a second copy: the other half of the next step's 2B-sample UNet input.
+// ------------------------------------------------------------------------------------------
+namespace pcm {
+__global__ void pcm_sample_step_kernel(const float* __restrict__ eps, const float* x,
+                                       float* x_out, float* x_out2, long long total, int cfg,
+                                       const double* __restrict__ guidance, double sa, double ss, double sap,
+                                       double ssp, int pred_type) {
+  griddep_sync();
+  const double g = cfg ? *guidance : 1.0;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    double e;
+    if (cfg) {
+      const double eu = eps[i], ec = eps[total + i];
+      e = eu + g * (ec - eu);
+    } else {
+      e = eps[i];
+    }
+    const double xv = x[i];
+    double x0, pe;
+    if (pred_type == 0) {
+      x0 = (xv - ss * e) / sa;
+      pe = e;
+    } else {
+      x0 = sa * xv - ss * e;
+      pe = sa * e + ss * xv;
+    }
+    const float o = static_cast<float>(sap * x0 + ssp * pe);
+    x_out[i] = o;
+    if (x_out2) x_out2[i] = o;
+  }
+}
+}  // namespace pcm
+
+extern "C" int pcm_sample_step(const float* eps, const float* x, float* x_out, float* x_out2, int64_t per,
+                               int B, int cfg, const double* guidance, double sqrt_a_t, double sqrt_1m_a_t,
+                               double sqrt_a_prev, double sqrt_1m_a_prev, int pred_type, void* stream) {
+  if (pred_type != 0 && pred_type != 1) return set_error("pcm_sample_step: bad prediction type");
+  if (cfg && !guidance) return set_error("pcm_sample_step: guidance needs its device scalar");
+  const long long total = per * B;
+  CUDA_TRY(launch_pdl(pcm_sample_step_kernel, dim3(grid_for(total)), dim3(256), 0, ST(stream), eps, x, x_out,
+                      x_out2, total, cfg ? 1 : 0, guidance, sqrt_a_t, sqrt_1m_a_t, sqrt_a_prev,
+                      sqrt_1m_a_prev, pred_type));
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
 extern "C" int pcm_teacher_substep(const float* eps_c, const float* eps_u, const float* x_cur,
                                    const float* alphas_cumprod, const int64_t* t_cur,
                                    const int64_t* t_next, const double* coef, int64_t per, int B,

@@ -393,3 +393,23 @@ def colsum(x, out, B, HW):
 def add_bf16(a, b, out):
     _call("pcm_add_bf16", _p(a), _p(b), a.numel(), _p(out))
     return out
+
+
+def lora_fuse(master, table, work, scale):
+    """W + scale * B A into the destinations of `table` (UNetB200.fused_inference_net), from the fp32
+    masters `master`."""
+    assert master.dtype == torch.float32 and table.dtype == torch.int64 and table.shape[1] == 8
+    _call("pcm_lora_fuse", _p(master), _p(table), table.shape[0], work, scale)
+
+
+def sample_step(eps, x, out, out2, guidance, sa, ss, sap, ssp, pred_type):
+    """One eta = 0 DDIM step on fp32 latents x [B, ...].  guidance: None, or a float64 device scalar g
+    (eps is then the [uncond; cond] batch [2B, ...], mixed eps_u + g (eps_c - eps_u))."""
+    B = x.shape[0]
+    per = x.numel() // B
+    cfg = guidance is not None
+    assert eps.shape[0] == (2 * B if cfg else B) and eps.dtype == x.dtype == torch.float32
+    assert not cfg or guidance.dtype == torch.float64
+    _call("pcm_sample_step", _p(eps), _p(x), _p(out), _p(out2), per, B, int(cfg), _p(guidance), sa, ss, sap,
+          ssp, pred_type)
+    return out

@@ -100,6 +100,10 @@ def parse_args(argv=None, extra=None):
                    help="noise_scheduler.config.prediction_type of the teacher (T15:1204, 1228)")
     p.add_argument("--ema_decay", type=float, default=None,
                    help="opt-in EMA target (update_ema, T15:344-355); default: target = student like the reference")
+    p.add_argument("--validation_prompt_embeds", type=str, default=None,
+                   help=".pt dict {prompt_embeds [P,77,D]} (+ text_embeds [P,*], time_ids [P or 1,6] for SDXL): "
+                        "sample 4 images per prompt in --multiphase steps every --validation_steps (T15:1345-1365) "
+                        "into output_dir/validation/step-N/cfg-{g}.pt")
     args = p.parse_args(argv)
     env_local_rank = int(os.environ.get("LOCAL_RANK", -1))   # same override as the reference
     if env_local_rank != -1 and env_local_rank != args.local_rank:
@@ -175,6 +179,64 @@ def load_state(st, path, gen):
     st.load_state_dict(sd)
     gen.set_state(sd["rng_state"])
     return int(sd["global_step"])
+
+
+def validation_enabled(args):
+    """Validation sampling is opt-in: it runs only with --validation_prompt_embeds."""
+    return args.validation_prompt_embeds is not None
+
+
+def validation_guidances(config_sdxl):
+    """log_validation's guidance scales: 1 and 7.5 for SD1.5 (T15:1345-1365), 1 for SDXL (TXL:1578)."""
+    return (1.0,) if config_sdxl else (1.0, 7.5)
+
+
+class _Validation:
+    """log_validation (T15:120-207) on latents: the LoRA fused into an inference copy of the UNet, each
+    prompt sampled 4 times in `multiphase` DDIM-trailing steps from one generator seeded with --seed, at every
+    guidance scale; latents and seed saved to output_dir/validation/step-N/cfg-{g}.pt."""
+
+    def __init__(self, args, st, cfg, uncond):
+        d = torch.load(args.validation_prompt_embeds)
+        self.pe = d["prompt_embeds"].float().reshape(-1, 77, cfg.cross_attention_dim)
+        P = self.pe.shape[0]
+        self.ne = None if uncond is None else uncond.float().reshape(-1, 77, cfg.cross_attention_dim)[:1].repeat(P, 1, 1)
+        self.extra = {}
+        if cfg.addition_embed:
+            te = d["text_embeds"].float()
+            self.extra = dict(text_embeds=te, time_ids=d["time_ids"].long().reshape(-1, cfg.num_time_ids),
+                              negative_text_embeds=torch.zeros_like(te))
+        self.args, self.st, self.cfg = args, st, cfg
+        self.guidances = validation_guidances(cfg.addition_embed)
+        if any(g > 1 for g in self.guidances) and self.ne is None:
+            raise SystemExit("validation with guidance > 1 needs the empty-prompt embedding (--uncond_embeds)")
+        self.sampler = None
+
+    def __call__(self, global_step):
+        from .sampling import PCMSampler
+        if self.sampler is None:
+            self.sampler = PCMSampler(self.st.unet, alphas_cumprod=self.st.acp, prediction_type=self.args.prediction_type)
+        else:
+            self.sampler.fuse()
+        out_dir = os.path.join(self.args.output_dir, "validation", f"step-{global_step}")
+        os.makedirs(out_dir, exist_ok=True)
+        seed, res = self.args.seed, self.args.resolution
+        dev = self.st.unet.dev
+        for g in self.guidances:
+            gen = None if seed is None else torch.Generator(device=dev).manual_seed(seed)
+            lats = []
+            for i in range(self.pe.shape[0]):        # one pipeline call per prompt (T15:163-175)
+                ex = {}
+                if self.extra:
+                    tid = self.extra["time_ids"]
+                    ex = dict(text_embeds=self.extra["text_embeds"][i:i + 1],
+                              time_ids=tid[i:i + 1] if tid.shape[0] > 1 else tid,
+                              negative_text_embeds=self.extra["negative_text_embeds"][i:i + 1])
+                lats.append(self.sampler(self.pe[i:i + 1], None if self.ne is None else self.ne[i:i + 1],
+                                         num_inference_steps=self.args.multiphase, guidance_scale=g,
+                                         num_images_per_prompt=4, height=res, width=res, generator=gen, **ex))
+            torch.save({"latents": torch.cat(lats).cpu(), "seed": seed, "guidance_scale": g},
+                       os.path.join(out_dir, f"cfg-{g}.pt"))
 
 
 def main(args):
@@ -276,6 +338,7 @@ def main(args):
                 print(f"Resuming from checkpoint {path}")
             global_step = load_state(st, os.path.join(args.output_dir, path), gen)
             assert global_step == int(path.split("-")[1])
+    validate = _Validation(args, st, cfg, uncond) if rank == 0 and validation_enabled(args) else None
     gs = gen.get_state()                           # the capture / warm-up batch must not consume the
     st.load_inputs(*next_batch(global_step))       # data stream (resume == uninterrupted run)
     if not args.no_cuda_graph:
@@ -297,6 +360,8 @@ def main(args):
         if rank == 0 and global_step % args.checkpointing_steps == 0:
             rotate_checkpoints(args.output_dir, args.checkpoints_total_limit)
             save_state(st, cfg, os.path.join(args.output_dir, f"checkpoint-{global_step}"), global_step, gen)
+        if validate is not None and global_step % args.validation_steps == 0:
+            validate(global_step)
     if world > 1:
         torch.distributed.barrier()               # accelerator.wait_for_everyone()
     if rank == 0:

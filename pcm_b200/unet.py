@@ -474,6 +474,86 @@ class UNetB200:
         ops._call("pcm_lora_refresh", master.data_ptr(), self.refresh_table.data_ptr(),
                   self.refresh_table.shape[0], self.refresh_work, self.scale, self.lora_opnd.data_ptr())
 
+    def fused_inference_net(self):
+        """An inference network over this one's weights with the LoRA fused in (peft `fuse_lora`): no
+        backward, no LoRA operands, no tape.  Every K-blocked operand that holds a LoRA target's frozen
+        weight (single layers, the q/k/v stacks, the time_emb_proj stack, the cross-attention k / v
+        context chunks) gets a fused copy in ONE new bf16 buffer; every other tensor (norms, biases,
+        conv_in / conv_out, time embedding) is this network's own.  Returns (net, fuse_table, fuse_work):
+        fuse_table is the int64 [entries, 8] table of pcm_lora_fuse (ops.lora_fuse), one row per LoRA
+        layer: {a_off, b_off, src, dst, n0 | N_total << 32, K | r << 32, n, work_begin}."""
+        if not self.has_lora:
+            raise ValueError("fused_inference_net needs a network built with lora=True")
+        net = object.__new__(UNetB200)
+        net.__dict__.update(self.__dict__)
+        for k in ("lora_master", "lora_grad", "lora_opnd", "refresh_table", "refresh_work"):
+            net.__dict__.pop(k, None)
+        net.has_lora, net.use_wstream, net.wstream = False, False, None
+        net.gradient_checkpointing = False
+        net.lora_layers, net._keep, net._dkv_chunks = [], [], {}
+        net.saved = net._temb = net._ctxkv = net.last_ctx_kv = None
+        net._lb, net._plan_b = (1, 1), None
+        # stacked operands: (source, [(layer, first row)]) of every operand holding a LoRA target
+        stacks = []
+        for L in self.lora_layers:
+            if L.w_fwd is not None:     # not a member of a group: its own operand
+                stacks.append(("layer", L.name, L.w_fwd, [(L, 0)]))
+        for lead, G in self.groups.items():
+            if lead.endswith(".attn1.to_q"):
+                stacks.append(("group", lead, G.w_stack, [(L, i * G.cout) for i, L in enumerate(G.layers)]))
+        TG = self.temb_group
+        stacks.append(("temb", None, TG.w_stack, [(L, TG.offs[i]) for i, L in enumerate(TG.layers)]))
+        if self.ctx_group is not None:
+            for c, ch in enumerate(self.ctx_group.chunks):
+                Ls = [L for G in ch.blocks for L in G.layers]
+                stacks.append(("chunk", c, ch.w_stack, [(L, i * ch.cout) for i, L in enumerate(Ls)]))
+        total = sum(src.numel() for _, _, src, _ in stacks)
+        net.fused_weights = torch.empty(total, device=self.dev, dtype=BF16)
+        rows, work, off, fused = [], 0, 0, {}
+        for kind, key, src, members in stacks:
+            dst = net.fused_weights[off:off + src.numel()].view(src.shape)
+            off += src.numel()
+            fused[(kind, key)] = dst
+            K, ntot = src.shape[0] * 64, src.shape[1]
+            assert sum(L.cout for L, _ in members) == ntot     # every row of the operand is a LoRA layer's
+            for L, n0 in members:
+                taps = L.k * L.k if L.kind == "conv" else 1
+                assert L.lora is not None and taps * L.cin == K and L.cout % 64 == 0
+                rows.append([L.lora.a_off, L.lora.b_off, src.data_ptr(), dst.data_ptr(), n0 | (ntot << 32),
+                             K | (self.r << 32), L.cout, work])
+                work += (L.cout // 64) * (K // 64)
+        net.layers = {}
+        for name, L in self.layers.items():
+            C2 = _Layer()
+            for s in _Layer.__slots__:
+                setattr(C2, s, getattr(L, s))
+            C2.lora, C2.w_t = None, None
+            if ("layer", name) in fused:
+                C2.w_fwd = fused[("layer", name)]
+            net.layers[name] = C2
+        net.groups = {}
+        for lead, G in self.groups.items():
+            if not lead.endswith(".attn1.to_q"):
+                continue        # cross-attention k / v run as context chunks
+            G2 = types.SimpleNamespace(**vars(G))
+            G2.layers = [net.layers[n] for n in G.names]
+            G2.w_stack, G2.w_t_cat, G2.lora = fused[("group", lead)], None, False
+            net.groups[lead] = G2
+        T2 = types.SimpleNamespace(**vars(TG))
+        T2.layers = [net.layers[n] for n in TG.names]
+        T2.w_stack, T2.lora = fused[("temb", None)], False
+        net.temb_group = T2
+        if self.ctx_group is not None:
+            CG2 = types.SimpleNamespace(**vars(self.ctx_group))
+            CG2.lora, CG2.chunks = False, []
+            for c, ch in enumerate(self.ctx_group.chunks):
+                ch2 = types.SimpleNamespace(**vars(ch))
+                ch2.w_stack = fused[("chunk", c)]
+                CG2.chunks.append(ch2)
+            net.ctx_group = CG2
+        table = torch.tensor(rows, dtype=torch.int64, device=self.dev)
+        return net, table, work
+
     def block_grad_offsets(self):
         """First flat-buffer offset of every UNet block (resnet / transformer / resample conv) that owns
         LoRA layers, ascending - the bucket boundaries of the overlapped gradient all-reduce."""
