@@ -76,9 +76,11 @@ typedef struct {
   int32_t out_fp32, round_bf16;
   float alpha;
   int32_t act;           /* 0 none, 1 SiLU applied to the result */
-  int32_t ksplit;        /* > 1: split the K program over ksplit CTAs per tile (small-M, long-K) */
-  void* splitk_ws;       /* fp32 [ksplit, M, N] scratch: one slice of partial sums per K split, added in
-                            split order by the finalize kernel (required if ksplit > 1) */
+  int32_t ksplit;        /* > 1: split the K program over ksplit CTAs per tile (small-M, long-K).  A program
+                            with N-ranged entries runs unsplit whatever ksplit says (and then needs no
+                            workspace); otherwise ksplit > 1 without splitk_ws is an error */
+  void* splitk_ws;       /* fp32 [ksplit, M, N] scratch, 16-byte aligned: one slice of partial sums per K
+                            split, added in split order by the finalize kernel */
   int32_t dep_a_src1;    /* 1 + index of the ONLY A source written by the kernel launched immediately
                             before this one on the stream (the layer's LoRA down-projection T), 0 = none.
                             When set, the kernel starts under programmatic dependent launch without
@@ -118,9 +120,22 @@ const char* pcm_last_error(void);
 int pcm_version(void);
 int pcm_num_sms(void);
 
-/* wgmma implicit GEMM / conv and LoRA wgrad */
+/* wgmma implicit GEMM / conv and LoRA wgrad.  A descriptor the kernels cannot serve is rejected on the
+ * host before any CUDA call, pcm_last_error() naming the field: M, N < 1, a null out, conv mode with geoW,
+ * geoH, epiW or epiHW < 1, and alignment.  A launch with a bf16 output, no activation and no K split
+ * actually run (ksplit <= 1, N-ranged entries, or a program too short to split: ksplit is capped at one
+ * split per 64-wide K block) accesses memory 16 bytes at a time: with N >= 32, out, rowvec and bias must
+ * be 16-byte aligned and osW, osH, osB and rowvec_ld multiples of 8; with a residual and N >= 8, the
+ * residual must be 16-byte aligned and osW, osH, osB multiples of 8 (it is prefetched 8 columns at a
+ * time even where the stores are elementwise).  Every other access is elementwise and only needs the
+ * pointer aligned to its element.
+ * pcm_wgrad: M < 1, a null out, os_row or os_col of zero; out 4-byte aligned, and with os_col == 1 (ranks
+ * added in pairs) 8-byte aligned with even os_row and tap_off.
+ * pcm_gemm_check / pcm_wgrad_check run exactly those checks and launch nothing. */
 int pcm_gemm(const pcm_gemm_desc* d, void* stream);
 int pcm_wgrad(const pcm_wgrad_desc* d, void* stream);
+int pcm_gemm_check(const pcm_gemm_desc* d);
+int pcm_wgrad_check(const pcm_wgrad_desc* d);
 
 /* ---- GroupNorm(+SiLU) / LayerNorm (NHWC bf16; fp32 statistics) ----------------------------
  * Replace ATen group_norm/layer_norm/silu inside diffusers ResnetBlock2D / Transformer2DModel /

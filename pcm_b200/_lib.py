@@ -84,6 +84,8 @@ EXPORTS = [
     "pcm_num_sms",
     "pcm_gemm",
     "pcm_wgrad",
+    "pcm_gemm_check",
+    "pcm_wgrad_check",
     "pcm_groupnorm_ws_bytes",
     "pcm_groupnorm_fwd",
     "pcm_groupnorm_fwd_part",
@@ -122,6 +124,8 @@ P, I, L64, F, D = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
 ARGTYPES = {
     "pcm_gemm": [P, P],
     "pcm_wgrad": [P, P],
+    "pcm_gemm_check": [P],
+    "pcm_wgrad_check": [P],
     "pcm_groupnorm_ws_bytes": [I, I, I, I],
     "pcm_groupnorm_fwd": [P, P, I, I, I, I, I, P, P, F, I, P, P, P, L64, P],
     "pcm_groupnorm_fwd_part": [P, P, I, I, I, I, I, I, P, P, F, I, P, P, P, L64, P],

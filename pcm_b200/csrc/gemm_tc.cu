@@ -468,12 +468,94 @@ static GemmKernel gemm_kernel_for(int block_n) {
   }
 }
 
-static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
+// Descriptor checks, all on the host and before any CUDA or driver call: everything the kernels would
+// otherwise turn into a misaligned or wild access.  The fast epilogue (bf16 output, no activation, no
+// split-K, a full 32-column chunk) loads and stores 16 bytes at out / residual + row offset + n, at
+// rowvec + b * rowvec_ld + n and at bias + n with n % 8 == 0; every other path is elementwise.  The split-K
+// workspace is read and written as float4.
+static bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
+
+static bool gemm_ranged(const pcm_gemm_desc* d) {
+  for (int e = 0; e < d->num_prog; ++e)
+    if (d->prog[e].n_hi != 0) return true;
+  return false;
+}
+
+// The K split a launch runs: none for a program with N-ranged entries, at most one split per K block, and
+// no empty split.  One rule for the validation and the launch.
+static int gemm_ksplit(const pcm_gemm_desc* d) {
+  if (d->ksplit <= 1 || d->splitk_ws == nullptr || gemm_ranged(d)) return 1;
+  int nkb = 0;
+  for (int e = 0; e < d->num_prog; ++e) nkb += d->prog[e].nchunks;
+  if (nkb < 1) return 1;
+  const int ks = d->ksplit < nkb ? d->ksplit : nkb;
+  const int per = (nkb + ks - 1) / ks;
+  return (nkb + per - 1) / per;
+}
+
+static int validate_gemm(const pcm_gemm_desc* d) {
   if (d->block_n < 32 || d->block_n > 256 || (d->block_n % 32) != 0)
     return set_error("pcm_gemm: block_n must be a multiple of 32 in [32, 256]");
   if (d->num_a < 1 || d->num_a > PCM_MAX_ASRC || d->num_b < 1 || d->num_b > PCM_MAX_BSRC ||
       d->num_prog < 1 || d->num_prog > PCM_MAX_PROG)
     return set_error("pcm_gemm: bad source / program counts");
+  if (d->M < 1) return set_error("pcm_gemm: M must be >= 1");
+  if (d->N < 1) return set_error("pcm_gemm: N must be >= 1");
+  if (d->out == nullptr) return set_error("pcm_gemm: out is null");
+  if (!d->lin && (d->geoW < 1 || d->geoH < 1)) return set_error("pcm_gemm: geoW and geoH must be >= 1 in conv mode");
+  if (!d->lin && d->epiW < 1) return set_error("pcm_gemm: epiW must be >= 1 in conv mode");
+  if (!d->lin && d->epiHW < 1) return set_error("pcm_gemm: epiHW must be >= 1 in conv mode");
+  if (d->act != 0 && d->act != 1) return set_error("pcm_gemm: act must be 0 or 1");
+  if (d->dep_a_src1 < 0 || d->dep_a_src1 > d->num_a) return set_error("pcm_gemm: bad dep_a_src1");
+  if (d->ksplit > 1 && !gemm_ranged(d)) {
+    if (d->splitk_ws == nullptr) return set_error("pcm_gemm: ksplit > 1 needs splitk_ws");
+    if (misaligned(d->splitk_ws, 16)) return set_error("pcm_gemm: splitk_ws is not 16-byte aligned");
+  }
+  // the paths with 16-byte accesses: bf16 output, no activation, and the launch really runs unsplit
+  const bool wide = !d->out_fp32 && d->act == 0 && gemm_ksplit(d) == 1;
+  const bool vec = wide && d->N >= 32;   // a full 32-column chunk: out, bias, rowvec, residual by 16 bytes
+  // the residual prefetch reads 16 bytes wherever 8 columns fit, also in a ragged chunk
+  const bool vec_res = wide && d->residual != nullptr && d->N >= 8;
+  if (misaligned(d->out, vec ? 16 : (d->out_fp32 ? 4 : 2)))
+    return set_error(vec ? "pcm_gemm: out is not 16-byte aligned" : "pcm_gemm: out is not aligned to its element size");
+  if (d->bias && misaligned(d->bias, vec ? 16 : 4))
+    return set_error(vec ? "pcm_gemm: bias is not 16-byte aligned" : "pcm_gemm: bias is not 4-byte aligned");
+  if (d->rowvec && misaligned(d->rowvec, vec ? 16 : 2))
+    return set_error(vec ? "pcm_gemm: rowvec is not 16-byte aligned" : "pcm_gemm: rowvec is not 2-byte aligned");
+  if (d->residual && misaligned(d->residual, vec_res ? 16 : 2))
+    return set_error(vec_res ? "pcm_gemm: residual is not 16-byte aligned" : "pcm_gemm: residual is not 2-byte aligned");
+  if (vec || vec_res) {
+    if (d->osW % 8 != 0) return set_error("pcm_gemm: osW is not a multiple of 8");
+    if (d->osH % 8 != 0) return set_error("pcm_gemm: osH is not a multiple of 8");
+    if (d->osB % 8 != 0) return set_error("pcm_gemm: osB is not a multiple of 8");
+  }
+  if (vec && d->rowvec && d->rowvec_ld % 8 != 0) return set_error("pcm_gemm: rowvec_ld is not a multiple of 8");
+  return 0;
+}
+
+// The weight-gradient kernel adds pairs of ranks with one 8-byte reduction when os_col == 1.
+static int validate_wgrad(const pcm_wgrad_desc* d) {
+  if (d->M < 1) return set_error("pcm_wgrad: M must be >= 1");
+  if (d->out == nullptr) return set_error("pcm_wgrad: out is null");
+  if (d->os_row == 0) return set_error("pcm_wgrad: os_row is zero");
+  if (d->os_col == 0) return set_error("pcm_wgrad: os_col is zero");
+  if (d->num_taps < 1 || d->num_taps > 9) return set_error("pcm_wgrad: bad tap count");
+  if (!d->lin && (d->geoW < 1 || d->geoH < 1)) return set_error("pcm_wgrad: geoW and geoH must be >= 1 in conv mode");
+  const int qw = d->q.C - d->q_c0 < 64 ? d->q.C - d->q_c0 : 64;
+  if (d->q_c0 < 0 || qw < 8 || qw % 8 != 0)
+    return set_error("pcm_wgrad: the rank slice q[:, q_c0:] must hold a positive multiple of 8 columns");
+  const bool pairs = d->os_col == 1;
+  if (misaligned(d->out, pairs ? 8 : 4))
+    return set_error(pairs ? "pcm_wgrad: out is not 8-byte aligned" : "pcm_wgrad: out is not 4-byte aligned");
+  if (pairs && d->os_row % 2 != 0) return set_error("pcm_wgrad: os_row is odd with os_col == 1");
+  for (int t = 0; pairs && t < d->num_taps; ++t)
+    if (d->tap_off[t] % 2 != 0) return set_error("pcm_wgrad: tap_off is odd with os_col == 1");
+  if (d->sem && misaligned(d->sem, 4)) return set_error("pcm_wgrad: sem is not 4-byte aligned");
+  return 0;
+}
+
+static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
+  if (int rc = validate_gemm(d)) return rc;
   static GemmParams p;  // host staging (single host thread per rank)
   memset(&p, 0, sizeof(p));
   for (int i = 0; i < PCM_MAX_ASRC; ++i) {
@@ -554,16 +636,9 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
   p.round_bf16 = d->round_bf16;
   p.alpha = d->alpha;
   p.act = d->act;
-  p.ksplit = 1;
   p.ws = nullptr;
   p.dep_a_map = -1;
-  if (d->ksplit > 1 && d->splitk_ws != nullptr && !p.filtered) {
-    int ks = d->ksplit;
-    if (ks > nkb) ks = nkb;
-    const int per = (nkb + ks - 1) / ks;
-    ks = (nkb + per - 1) / per;  // every split non-empty
-    p.ksplit = ks;
-  }
+  p.ksplit = gemm_ksplit(d);   // (m_hi is only set for ksplit <= 1, so a split program is never filtered)
 
   const size_t smem = static_cast<size_t>(S) * stage_bytes + kStagingBytes + 1024;
   const GemmKernel kernel = narrow ? gemm_kernel_for<true>(d->block_n) : gemm_kernel_for<false>(d->block_n);
@@ -573,7 +648,6 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
     attr_set[narrow][d->block_n / 32] = true;
   }
   if (d->dep_a_src1 > 0 && p.ksplit == 1) {  // (split-K: the finalize kernel follows; keep the plain chain)
-    if (d->dep_a_src1 > d->num_a) return set_error("pcm_gemm: bad dep_a_src1");
     p.dep_a_map = d->dep_a_src1 - 1;
   }
   const int tiles = p.tiles_m * p.tiles_n * p.ksplit;
@@ -599,11 +673,11 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
 }
 
 static int launch_wgrad(const pcm_wgrad_desc* d, cudaStream_t stream) {
+  if (int rc = validate_wgrad(d)) return rc;
   static WgradParams p;
   memset(&p, 0, sizeof(p));
   if (int rc = encode_asrc(&p.p_map, d->p, d->lin, d->geoW, d->geoH)) return rc;
   if (int rc = encode_asrc(&p.q_map, d->q, d->lin, d->geoW, d->geoH)) return rc;
-  if (d->num_taps < 1 || d->num_taps > 9) return set_error("pcm_wgrad: bad tap count");
   p.lin = d->lin;
   p.geoW = d->lin ? 1 : d->geoW;
   p.geoHW = d->lin ? 1 : d->geoW * d->geoH;
@@ -611,8 +685,6 @@ static int launch_wgrad(const pcm_wgrad_desc* d, cudaStream_t stream) {
   p.Cp = d->p.C;
   p.q_c0 = d->q_c0;
   p.qw = d->q.C - d->q_c0 < 64 ? d->q.C - d->q_c0 : 64;
-  if (d->q_c0 < 0 || p.qw < 8 || p.qw % 8 != 0)
-    return set_error("pcm_wgrad: the rank slice q[:, q_c0:] must hold a positive multiple of 8 columns");
   p.num_taps = d->num_taps;
   for (int t = 0; t < d->num_taps; ++t) {
     p.dw[t] = d->dw[t];
@@ -658,6 +730,8 @@ static int launch_wgrad(const pcm_wgrad_desc* d, cudaStream_t stream) {
 extern "C" int pcm_gemm(const pcm_gemm_desc* d, void* stream) {
   return pcm::launch_gemm(d, reinterpret_cast<cudaStream_t>(stream));
 }
+extern "C" int pcm_gemm_check(const pcm_gemm_desc* d) { return pcm::validate_gemm(d); }
+extern "C" int pcm_wgrad_check(const pcm_wgrad_desc* d) { return pcm::validate_wgrad(d); }
 extern "C" int pcm_wgrad(const pcm_wgrad_desc* d, void* stream) {
   return pcm::launch_wgrad(d, reinterpret_cast<cudaStream_t>(stream));
 }
