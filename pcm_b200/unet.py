@@ -101,8 +101,36 @@ class _Lora:
 
 
 class _Layer:
-    __slots__ = ("name", "kind", "cin", "cout", "k", "w_fwd", "w_t", "bias", "gamma", "beta", "lora",
-                 "w_c4", "w_c4_t")
+    __slots__ = ("name", "kind", "cin", "cout", "k", "w_t", "bias", "gamma", "beta", "lora", "w_c4", "w_c4_t")
+
+
+# a frozen forward GEMM B operand: w = the bf16 weights of its member layers stacked along N, K-blocked
+# [K/64][N][64] (pcm_bsrc.kblocked), in a storage of its own; members = [(layer, its first row n0)]
+Operand = namedtuple("Operand", "w members")
+
+
+def _stacks(tab):
+    """The layers whose frozen weights are stacked along N into ONE forward operand because they read the
+    same input and run as one GEMM: [(operand key, kind, member names in row order)] for
+      * "qkv": the attn1 q / k / v of every transformer block (key: its to_q);
+      * "temb": every resnet's time_emb_proj, which read the same silu(temb) (1 base K entry + one N-ranged
+        LoRA entry per layer must fit the K program);
+      * "ctx": the cross-attention k / v of ALL transformer blocks, which read the same text context, in
+        chunks of at most 11 blocks of one width (22 N-ranged LoRA entries + the base entry <= PCM_MAX_PROG)."""
+    names = [n for n, *_ in tab]
+    out = [(n, "qkv", [n[:-1] + c for c in "qkv"]) for n in names if n.endswith(".attn1.to_q")]
+    temb = [n for n in names if n.endswith(".time_emb_proj")]
+    if len(temb) > 23:
+        raise ValueError(f"{len(temb)} time_emb_proj layers: the grouped time-embedding GEMM holds at most 23 "
+                         f"(PCM_MAX_PROG - 1)")
+    out.append(("temb", "temb", temb))
+    co = {n: c for n, _, _, c, _ in tab}
+    chunks = []
+    for n in sorted((n for n in names if n.endswith(".attn2.to_k")), key=co.get):   # stable: one width together
+        if not chunks or co[chunks[-1][0]] != co[n] or len(chunks[-1]) == 22:
+            chunks.append([])
+        chunks[-1] += [n, n[:-1] + "v"]
+    return out + [(f"ctx.{c}", "ctx", ch) for c, ch in enumerate(chunks)]
 
 
 class UNetB200:
@@ -121,24 +149,16 @@ class UNetB200:
         self.layers = {}
         self.has_lora = lora
         tab = layer_table(cfg)
-        # every resnet's time_emb_proj reads the same silu(temb): one grouped GEMM per pass
-        # (1 base K entry + one N-ranged LoRA entry per layer must fit the K program)
-        self._temb_names = [n for n, *_ in tab if n.endswith(".time_emb_proj")]
-        if len(self._temb_names) > 23:
-            raise ValueError(f"{len(self._temb_names)} time_emb_proj layers: the grouped time-embedding GEMM "
-                             f"holds at most 23 (PCM_MAX_PROG - 1)")
-        # every cross-attention k / v projection reads the same text context: a few grouped GEMMs per
-        # pass (chunks of <= 11 transformer blocks of one width, _build_ctx_group) instead of one per block
-        self._ctx_names = [n for n, *_ in tab if n.endswith((".attn2.to_k", ".attn2.to_v"))]
-        _co = {n: co for n, _, _, co, _ in tab}
-        self._ctx_names.sort(key=lambda n: _co[n])        # stable: blocks of one width become neighbours
+        stacks = _stacks(tab)
+        stacked = {n for _, _, names in stacks for n in names}
+        # every cross-attention k / v layer, chunk after chunk: one LoRA down-projection serves all chunks
+        self._ctx_names = [n for _, kind, names in stacks if kind == "ctx" for n in names]
         master, entries, opnd_total = [], [], 0
         moff = 0
-        no_dgrad = ("attn2.to_k", "attn2.to_v", "time_emb_proj")
         for name, kind, cin, cout, k in tab:
             L = _Layer()
             L.name, L.kind, L.cin, L.cout, L.k = name, kind, cin, cout, k
-            L.w_fwd = L.w_t = L.bias = L.gamma = L.beta = L.lora = L.w_c4 = L.w_c4_t = None
+            L.w_t = L.bias = L.gamma = L.beta = L.lora = L.w_c4 = L.w_c4_t = None
             if kind in ("gn", "ln"):
                 L.gamma = state_dict[name + ".weight"].float().to(device)
                 L.beta = state_dict[name + ".bias"].float().to(device)
@@ -147,20 +167,17 @@ class UNetB200:
             W = state_dict[name + ".weight"].float()
             if (name + ".bias") in state_dict:
                 L.bias = state_dict[name + ".bias"].float().to(device)
-            if kind == "conv":
-                if name == "conv_in":
-                    L.w_c4 = W.permute(0, 2, 3, 1).contiguous().to(device=device, dtype=BF16)  # [C][3][3][4]
-                else:
-                    L.w_fwd = W.permute(0, 2, 3, 1).reshape(cout, -1).contiguous().to(device=device, dtype=BF16)
-                    if name == "conv_out":
-                        L.w_c4_t = W.permute(1, 2, 3, 0).contiguous().to(device=device, dtype=BF16)  # [C][3][3][4]
-                    elif need_backward:
-                        L.w_t = W.permute(1, 2, 3, 0).reshape(cin, -1).contiguous().to(device=device, dtype=BF16)
-            else:
-                L.w_fwd = W.contiguous().to(device=device, dtype=BF16)
-                if need_backward and not name.endswith(no_dgrad) and \
-                        not name.startswith(("time_embedding", "add_embedding")):
-                    L.w_t = W.t().contiguous().to(device=device, dtype=BF16)
+            if name == "conv_in":
+                L.w_c4 = W.permute(0, 2, 3, 1).contiguous().to(device=device, dtype=BF16)  # [C][3][3][4]
+            elif name == "conv_out":
+                L.w_c4_t = W.permute(1, 2, 3, 0).contiguous().to(device=device, dtype=BF16)  # [C][3][3][4]
+            elif kind == "conv":
+                if need_backward:
+                    L.w_t = self._kblocked(W.permute(1, 2, 3, 0).reshape(cin, -1))
+            # no input gradient through the (frozen) time embedding, nor per stacked layer: time_emb_proj and
+            # the cross-attention k / v read inputs nothing trains, q / k / v run one dgrad over the group
+            elif need_backward and name not in stacked and not name.startswith(("time_embedding", "add_embedding")):
+                L.w_t = self._kblocked(W.t())
             if lora and is_lora_target(name):
                 taps = k * k if kind == "conv" else 1
                 A = state_dict[name + ".lora_A.weight"].float()
@@ -186,15 +203,16 @@ class UNetB200:
             self.lora_master = torch.cat(master).to(device)
             self.lora_grad = torch.zeros_like(self.lora_master)
             self.lora_opnd = torch.empty(opnd_total, device=device, dtype=BF16)
-            # operand copies: [A | s*B | (s*B)^T | A^T] per layer; the layers of a shared-input group
-            # (attn1 q/k/v, attn2 k/v) are laid out kind-major so that their A, s*B and (s*B)^T
-            # copies stack into single GEMM operands
+            # operand copies: [A | s*B | (s*B)^T | A^T] per layer; the layers of a stack are laid out
+            # kind-major so that their A, s*B and (s*B)^T copies stack into single GEMM operands, and so are
+            # the cross-attention k / v layers of ALL chunks: one down-projection serves every chunk
+            unit_of = {n: self._ctx_names if kind == "ctx" else names for _, kind, names in stacks for n in names}
             by_name = {L.name: (L, taps) for L, taps in entries}
             units, seen = [], set()
             for L, taps in entries:
                 if L.name in seen:
                     continue
-                grp = self._unit_of(L.name)
+                grp = unit_of.get(L.name)
                 members = [by_name[n] for n in grp] if grp and all(n in by_name for n in grp) else [(L, taps)]
                 seen.update(m[0].name for m in members)
                 units.append(members)
@@ -225,10 +243,10 @@ class UNetB200:
             self.refresh_table = torch.tensor(rows, dtype=torch.int64, device=device)
             self.refresh_work = work
             self.refresh_lora()
-        self._build_groups(need_backward)
-        self._build_temb_group()
-        self._build_ctx_group()
-        self._block_weights()
+        self._build_operands(state_dict, tab, stacks, stacked)
+        self._build_groups(state_dict, stacks, need_backward)
+        self._build_temb_group(next(names for _, kind, names in stacks if kind == "temb"))
+        self._build_ctx_group([(key, names) for key, kind, names in stacks if kind == "ctx"])
         self.saved = None
         self._temb = None
         self._ctxkv = self.last_ctx_kv = None
@@ -243,26 +261,27 @@ class UNetB200:
         self.wstream = torch.cuda.Stream(device=device) if self.use_wstream else None
         self._keep = []
 
-    _GROUPS = ((".attn1.to_q", (".attn1.to_q", ".attn1.to_k", ".attn1.to_v")),
-               (".attn2.to_k", (".attn2.to_k", ".attn2.to_v")))
+    def _kblocked(self, W):
+        """bf16 copy of the fp32 [N, K] matrix W on the device, K-blocked [K/64][N][64] (pcm_bsrc.kblocked):
+        the operand tile of a K block is one contiguous run in HBM.  Matters for the small-M layers (8x8 /
+        16x16 levels, target pass), which stream their weights once per launch: a row-major tile is N
+        separate 128-byte segments K*2 bytes apart."""
+        return ops.kblock(W.to(device=self.dev, dtype=BF16))
 
-    def _group_of(self, name):
-        """Names of the shared-input Linear group `name` belongs to (attn1 q/k/v, attn2 k/v, all
-        time_emb_proj layers), or None."""
-        if name.endswith(".time_emb_proj"):
-            return self._temb_names
-        for _, sufs in self._GROUPS:
-            for suf in sufs:
-                if name.endswith(suf):
-                    return [name[:-len(suf)] + x for x in sufs]
-        return None
-
-    def _unit_of(self, name):
-        """Layers whose LoRA operand copies are laid out kind-major next to each other: the shared-input
-        group of `name`, widened to ALL cross-attention k / v layers (they run as context chunks)."""
-        if name.endswith((".attn2.to_k", ".attn2.to_v")):
-            return self._ctx_names
-        return self._group_of(name)
+    def _build_operands(self, state_dict, tab, stacks, stacked):
+        """self.operands = {key: Operand}: the forward B operand of every GEMM that reads a frozen weight,
+        built once from the state dict.  Every Linear / 1x1 / 3x3 layer outside a stack has its own (key:
+        the layer name), then come the stacks of _stacks.  conv_in runs its own 4-channel kernel on w_c4."""
+        single = [(n, [n]) for n, kind, *_ in tab if kind not in ("gn", "ln") and n != "conv_in" and n not in stacked]
+        self.operands = {}
+        for key, names in single + [(key, names) for key, _, names in stacks]:
+            Ls = [self.layers[n] for n in names]
+            rows = []
+            for L in Ls:
+                W = state_dict[L.name + ".weight"].float()
+                rows.append(W.permute(0, 2, 3, 1).reshape(L.cout, -1) if L.kind == "conv" else W)  # [N, taps*cin]
+            n0 = [sum(L.cout for L in Ls[:i]) for i in range(len(Ls))]
+            self.operands[key] = Operand(self._kblocked(torch.cat(rows)), list(zip(Ls, n0)))
 
     def _stacked(self, layers, kind, rows, cols):
         """The `kind` ("a_fwd", "sb_fwd", "sb_t") operand copies of `layers`, laid out kind-major next to
@@ -273,38 +292,35 @@ class UNetB200:
         assert last.data_ptr() == v.view(-1)[-last.numel():].data_ptr()
         return v
 
-    def _build_groups(self, need_backward):
-        """Stack the frozen weights (and view the kind-major LoRA operand copies) of every shared-input
-        group so that q/k/v (resp. cross-attention k/v) run as ONE GEMM with N = g*C."""
+    def _build_groups(self, state_dict, stacks, need_backward):
+        """self.groups, keyed by their first layer: the shared-input Linear groups, whose LoRA operand copies
+        are viewed as stacks so that their LoRA K blocks enter one GEMM.  The q / k / v of a transformer
+        block run forward as ONE GEMM over their stacked operand (N = 3C) and backward as one dgrad GEMM
+        over w_t_cat [cin, 3C]; the cross-attention k / v of one block run forward in a context chunk and
+        backward only into their LoRA weight gradients."""
         self.groups = {}
-        for name in list(self.layers):
-            for lead, _ in self._GROUPS:
-                if not name.endswith(lead):
-                    continue
-                names = self._group_of(name)
-                Ls = [self.layers[n] for n in names]
-                assert all(L.bias is None and L.cin == Ls[0].cin and L.cout == Ls[0].cout for L in Ls)
-                G = types.SimpleNamespace(names=names, layers=Ls, g=len(Ls), cin=Ls[0].cin, cout=Ls[0].cout)
-                G.w_stack = torch.cat([L.w_fwd for L in Ls], 0).contiguous()
-                G.w_t_cat = None
-                if all(L.w_t is not None for L in Ls):
-                    G.w_t_cat = torch.cat([L.w_t for L in Ls], 1).contiguous()   # [cin, g*C]
-                for i, L in enumerate(Ls):
-                    L.w_fwd = G.w_stack[i * G.cout:(i + 1) * G.cout]
-                    L.w_t = None
-                G.lora = all(L.lora is not None for L in Ls)
-                if G.lora:
-                    r, g = self.r, G.g
-                    G.a_stack = self._stacked(Ls, "a_fwd", g * r, G.cin)
-                    G.sb_stack = self._stacked(Ls, "sb_fwd", g * G.cout, r)
-                    G.sbt_stack = self._stacked(Ls, "sb_t", g * r, G.cout)
-                self.groups[name] = G
+        qkv = [(names, need_backward) for _, kind, names in stacks if kind == "qkv"]
+        kv = [(names[i:i + 2], False) for _, kind, names in stacks if kind == "ctx" for i in range(0, len(names), 2)]
+        for names, dgrad in qkv + kv:
+            Ls = [self.layers[n] for n in names]
+            assert all(L.bias is None and L.cin == Ls[0].cin and L.cout == Ls[0].cout for L in Ls)
+            G = types.SimpleNamespace(names=names, layers=Ls, g=len(Ls), cin=Ls[0].cin, cout=Ls[0].cout)
+            G.w_t_cat = None
+            if dgrad:       # [cin, g*C]
+                G.w_t_cat = self._kblocked(torch.cat([state_dict[n + ".weight"].float() for n in names]).t())
+            G.lora = all(L.lora is not None for L in Ls)
+            if G.lora:
+                r, g = self.r, G.g
+                G.a_stack = self._stacked(Ls, "a_fwd", g * r, G.cin)
+                G.sb_stack = self._stacked(Ls, "sb_fwd", g * G.cout, r)
+                G.sbt_stack = self._stacked(Ls, "sb_t", g * r, G.cout)
+            self.groups[names[0]] = G
 
-    def _build_temb_group(self):
-        """Stacked operands of the time-embedding projections: W [sum C_i, temb], bias [sum C_i] and
-        the kind-major LoRA copies A [g*r, temb], s*B [sum C_i, r]."""
-        Ls = [self.layers[n] for n in self._temb_names]
-        G = types.SimpleNamespace(names=self._temb_names, layers=Ls, g=len(Ls), cin=Ls[0].cin)
+    def _build_temb_group(self, names):
+        """The time-embedding projections, which run as ONE GEMM over the "temb" operand: column offsets,
+        bias [sum C_i] and the kind-major LoRA copies A [g*r, temb], s*B [sum C_i, r]."""
+        Ls = [self.layers[n] for n in names]
+        G = types.SimpleNamespace(names=names, layers=Ls, g=len(Ls), cin=Ls[0].cin)
         assert all(L.cin == G.cin and L.bias is not None for L in Ls)
         G.offs = [0]
         for L in Ls:
@@ -313,10 +329,7 @@ class UNetB200:
         assert G.n_total < 65536
         G.bn = 160 if all(o % 160 == 0 for o in G.offs) else 64
         G.index = {n: i for i, n in enumerate(G.names)}
-        G.w_stack = torch.cat([L.w_fwd for L in Ls], 0).contiguous()
         G.bias = torch.cat([L.bias for L in Ls]).contiguous()
-        for i, L in enumerate(Ls):
-            L.w_fwd = G.w_stack[G.offs[i]:G.offs[i + 1]]
         G.lora = all(L.lora is not None for L in Ls)
         if G.lora:
             G.a_stack = self._stacked(Ls, "a_fwd", G.g * self.r, G.cin)
@@ -351,43 +364,38 @@ class UNetB200:
         column block i of T for its LoRA weight gradients."""
         G, r = self.temb_group, self.r
         T = self._lora_down(st[:self._lrows(st.shape[0])], G.a_stack) if lora and G.lora else None
-        out = self._stacked_gemm(st, G.w_stack, T, getattr(G, "sb_stack", None),
+        out = self._stacked_gemm(st, self.operands["temb"].w, T, getattr(G, "sb_stack", None),
                                  [(i * r, G.offs[i], G.offs[i + 1]) for i in range(G.g)], G.n_total,
                                  block_n=G.bn, bias=G.bias)
         return out, T
 
-    def _build_ctx_group(self):
+    def _build_ctx_group(self, chunks):
         """Cross-attention k / v of ALL transformer blocks from the text context (they depend on nothing
-        else): A copies of every layer stacked [n_layers*r, ctx_dim] for ONE down-projection GEMM, and the
-        frozen weights + s*B copies stacked per chunk (blocks of one width, at most 11 blocks = 22 N-ranged
-        LoRA entries + the base entry <= PCM_MAX_PROG)."""
+        else), chunks = [(operand key, member names)]: A copies of every layer stacked [n_layers*r, ctx_dim]
+        for ONE down-projection GEMM, and per chunk the s*B copies stacked like its frozen operand."""
         self.ctx_group = None
-        if not self._ctx_names:
+        if not chunks:
             return
         names = self._ctx_names
         Ls = [self.layers[n] for n in names]
-        assert all(L.bias is None and L.cin == Ls[0].cin for L in Ls) and len(names) % 2 == 0
+        assert all(L.bias is None and L.cin == Ls[0].cin for L in Ls)
         CG = types.SimpleNamespace(names=names, cin=Ls[0].cin, nl=len(names), chunks=[], where={})
         CG.lora = all(L.lora is not None for L in Ls)
         if CG.lora:
             CG.a_stack = self._stacked(Ls, "a_fwd", CG.nl * self.r, CG.cin)
-        cur = None
-        for b in range(len(names) // 2):
-            lead = names[2 * b]
-            assert lead.endswith(".attn2.to_k") and names[2 * b + 1] == lead[:-1] + "v"
-            G = self.groups[lead]
-            if cur is None or cur.cout != G.cout or len(cur.blocks) == 11:
-                cur = types.SimpleNamespace(cout=G.cout, blocks=[], first=2 * b)
-                CG.chunks.append(cur)
-            CG.where[lead[:-len(".attn2.to_k")]] = (len(CG.chunks) - 1, len(cur.blocks))
-            cur.blocks.append(G)
-        for ch in CG.chunks:
-            ch.n_total = 2 * ch.cout * len(ch.blocks)
+        first = 0
+        for key, ch_names in chunks:
+            blocks = [self.groups[n] for n in ch_names[::2]]
+            ch = types.SimpleNamespace(key=key, cout=blocks[0].cout, blocks=blocks, first=first)
+            ch.n_total = 2 * ch.cout * len(blocks)
             assert ch.n_total < 65536
             ch.bn = 160 if ch.cout % 160 == 0 else 64
-            ch.w_stack = torch.cat([G.w_stack for G in ch.blocks], 0).contiguous()
             if CG.lora:
-                ch.sb_stack = self._stacked([L for G in ch.blocks for L in G.layers], "sb_fwd", ch.n_total, self.r)
+                ch.sb_stack = self._stacked([L for G in blocks for L in G.layers], "sb_fwd", ch.n_total, self.r)
+            for j, G in enumerate(blocks):
+                CG.where[G.names[0][:-len(".attn2.to_k")]] = (len(CG.chunks), j)
+            CG.chunks.append(ch)
+            first += len(ch_names)
         self.ctx_group = CG
 
     def ctx_kv_all(self, ctx, lora):
@@ -395,7 +403,7 @@ class UNetB200:
         T the block's two columns blocks [Ml, 2r] of the stacked LoRA down-projection (None without LoRA)."""
         CG, r = self.ctx_group, self.r
         T = self._lora_down(ctx[:self._lrows(ctx.shape[0])], CG.a_stack) if lora and CG.lora else None
-        outs = [self._stacked_gemm(ctx, ch.w_stack, T, getattr(ch, "sb_stack", None),
+        outs = [self._stacked_gemm(ctx, self.operands[ch.key].w, T, getattr(ch, "sb_stack", None),
                                    [((ch.first + i) * r, i * ch.cout, (i + 1) * ch.cout)
                                     for i in range(2 * len(ch.blocks))], ch.n_total, block_n=ch.bn)
                 for ch in CG.chunks]
@@ -412,29 +420,6 @@ class UNetB200:
         """The leading `rows` context rows of a ctx_kv_all result (k / v only): the student samples'
         projections of the merged pass, reused by the target pass (same context, same weights)."""
         return {t: (k[:rows], v[:rows], None) for t, (k, v, _) in kv.items()}
-
-    def _block_weights(self):
-        """Store every frozen GEMM weight K-blocked ([K/64][N][64], pcm_bsrc.kblocked): the operand tile of
-        a K block becomes one contiguous run in HBM.  Matters for the small-M layers (8x8 / 16x16 levels,
-        target pass), which stream their weights once per launch: a row-major tile is N separate
-        128-byte segments K*2 bytes apart."""
-        members = set()
-        for G in list(self.groups.values()) + [self.temb_group]:
-            members.update(id(L) for L in G.layers)
-            G.w_stack = ops.kblock(G.w_stack)
-            if getattr(G, "w_t_cat", None) is not None:
-                G.w_t_cat = ops.kblock(G.w_t_cat)
-        if self.ctx_group is not None:
-            for ch in self.ctx_group.chunks:
-                ch.w_stack = ops.kblock(ch.w_stack)
-        for L in self.layers.values():
-            if id(L) in members:
-                L.w_fwd = None          # only reachable through the group's stacked operand
-                continue
-            if L.w_fwd is not None and L.w_fwd.dim() == 2:
-                L.w_fwd = ops.kblock(L.w_fwd)
-            if L.w_t is not None and L.w_t.dim() == 2:
-                L.w_t = ops.kblock(L.w_t)
 
     class _Side:
         """Run the enclosed launches on the wgrad side stream, ordered after everything enqueued so far
@@ -476,12 +461,13 @@ class UNetB200:
 
     def fused_inference_net(self):
         """An inference network over this one's weights with the LoRA fused in (peft `fuse_lora`): no
-        backward, no LoRA operands, no tape.  Every K-blocked operand that holds a LoRA target's frozen
-        weight (single layers, the q/k/v stacks, the time_emb_proj stack, the cross-attention k / v
-        context chunks) gets a fused copy in ONE new bf16 buffer; every other tensor (norms, biases,
-        conv_in / conv_out, time embedding) is this network's own.  Returns (net, fuse_table, fuse_work):
-        fuse_table is the int64 [entries, 8] table of pcm_lora_fuse (ops.lora_fuse), one row per LoRA
-        layer: {a_off, b_off, src, dst, n0 | N_total << 32, K | r << 32, n, work_begin}."""
+        backward, no LoRA operands, no tape.  Every operand of self.operands whose layers are LoRA targets
+        (single layers, the q/k/v stacks, the time_emb_proj stack, the cross-attention k / v context
+        chunks) gets a fused copy in ONE new bf16 buffer, net.fused_weights; net.operands points there.
+        Everything else (layers, groups, norms, biases, the other operands) is this network's own.
+        Returns (net, fuse_table, fuse_work): fuse_table is the int64 [entries, 8] table of pcm_lora_fuse
+        (ops.lora_fuse), one row per LoRA layer: {a_off, b_off, src, dst, n0 | N_total << 32, K | r << 32,
+        n, work_begin}."""
         if not self.has_lora:
             raise ValueError("fused_inference_net needs a network built with lora=True")
         net = object.__new__(UNetB200)
@@ -493,64 +479,21 @@ class UNetB200:
         net.lora_layers, net._keep, net._dkv_chunks = [], [], {}
         net.saved = net._temb = net._ctxkv = net.last_ctx_kv = None
         net._lb, net._plan_b = (1, 1), None
-        # stacked operands: (source, [(layer, first row)]) of every operand holding a LoRA target
-        stacks = []
-        for L in self.lora_layers:
-            if L.w_fwd is not None:     # not a member of a group: its own operand
-                stacks.append(("layer", L.name, L.w_fwd, [(L, 0)]))
-        for lead, G in self.groups.items():
-            if lead.endswith(".attn1.to_q"):
-                stacks.append(("group", lead, G.w_stack, [(L, i * G.cout) for i, L in enumerate(G.layers)]))
-        TG = self.temb_group
-        stacks.append(("temb", None, TG.w_stack, [(L, TG.offs[i]) for i, L in enumerate(TG.layers)]))
-        if self.ctx_group is not None:
-            for c, ch in enumerate(self.ctx_group.chunks):
-                Ls = [L for G in ch.blocks for L in G.layers]
-                stacks.append(("chunk", c, ch.w_stack, [(L, i * ch.cout) for i, L in enumerate(Ls)]))
-        total = sum(src.numel() for _, _, src, _ in stacks)
-        net.fused_weights = torch.empty(total, device=self.dev, dtype=BF16)
-        rows, work, off, fused = [], 0, 0, {}
-        for kind, key, src, members in stacks:
+        fused = {key: op for key, op in self.operands.items() if any(L.lora is not None for L, _ in op.members)}
+        net.fused_weights = torch.empty(sum(op.w.numel() for op in fused.values()), device=self.dev, dtype=BF16)
+        net.operands = dict(self.operands)
+        rows, work, off = [], 0, 0
+        for key, (src, members) in fused.items():
             dst = net.fused_weights[off:off + src.numel()].view(src.shape)
             off += src.numel()
-            fused[(kind, key)] = dst
+            net.operands[key] = Operand(dst, members)
             K, ntot = src.shape[0] * 64, src.shape[1]
-            assert sum(L.cout for L, _ in members) == ntot     # every row of the operand is a LoRA layer's
             for L, n0 in members:
                 taps = L.k * L.k if L.kind == "conv" else 1
                 assert L.lora is not None and taps * L.cin == K and L.cout % 64 == 0
                 rows.append([L.lora.a_off, L.lora.b_off, src.data_ptr(), dst.data_ptr(), n0 | (ntot << 32),
                              K | (self.r << 32), L.cout, work])
                 work += (L.cout // 64) * (K // 64)
-        net.layers = {}
-        for name, L in self.layers.items():
-            C2 = _Layer()
-            for s in _Layer.__slots__:
-                setattr(C2, s, getattr(L, s))
-            C2.lora, C2.w_t = None, None
-            if ("layer", name) in fused:
-                C2.w_fwd = fused[("layer", name)]
-            net.layers[name] = C2
-        net.groups = {}
-        for lead, G in self.groups.items():
-            if not lead.endswith(".attn1.to_q"):
-                continue        # cross-attention k / v run as context chunks
-            G2 = types.SimpleNamespace(**vars(G))
-            G2.layers = [net.layers[n] for n in G.names]
-            G2.w_stack, G2.w_t_cat, G2.lora = fused[("group", lead)], None, False
-            net.groups[lead] = G2
-        T2 = types.SimpleNamespace(**vars(TG))
-        T2.layers = [net.layers[n] for n in TG.names]
-        T2.w_stack, T2.lora = fused[("temb", None)], False
-        net.temb_group = T2
-        if self.ctx_group is not None:
-            CG2 = types.SimpleNamespace(**vars(self.ctx_group))
-            CG2.lora, CG2.chunks = False, []
-            for c, ch in enumerate(self.ctx_group.chunks):
-                ch2 = types.SimpleNamespace(**vars(ch))
-                ch2.w_stack = fused[("chunk", c)]
-                CG2.chunks.append(ch2)
-            net.ctx_group = CG2
         table = torch.tensor(rows, dtype=torch.int64, device=self.dev)
         return net, table, work
 
@@ -647,7 +590,7 @@ class UNetB200:
         Ho, Wo = H // stride, W // stride
         M, N = B * Ho * Wo, L.cout
         srcs, prog = self._conv_prog(xs, 3, stride, L.cin)
-        bs = [ops.bsrc(L.w_fwd)]
+        bs = [ops.bsrc(self.operands[name].w)]
         T = None
         lbn = self._lrows(B)   # samples that carry the LoRA adapter (the leading ones of the batch)
         xl = xs if lbn == B else [x[:lbn] for x in xs]
@@ -679,7 +622,7 @@ class UNetB200:
         for si, x in enumerate(xs):
             prog.append((si, 0, 0, 0, x.shape[1] // 64, 0, coff))
             coff += x.shape[1]
-        bs = [ops.bsrc(L.w_fwd)]
+        bs = [ops.bsrc(self.operands[name].w)]
         T = None
         Ml = self._lrows(M)
         xl = xs if Ml == M else [x[:Ml] for x in xs]
@@ -706,7 +649,7 @@ class UNetB200:
         g, Cc = G.g, G.cout
         xl = x[:self._lrows(x.shape[0])]
         T = self._lora_down(xl, G.a_stack) if lora and G.lora else None
-        out = self._stacked_gemm(x, G.w_stack, T, getattr(G, "sb_stack", None),
+        out = self._stacked_gemm(x, self.operands[lead].w, T, getattr(G, "sb_stack", None),
                                  [(i * r, i * Cc, (i + 1) * Cc) for i in range(g)], g * Cc,
                                  block_n=160 if Cc % 160 == 0 else 64, dep_a_src=None if T is None else 1)
         if save is not None:

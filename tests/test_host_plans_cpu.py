@@ -105,23 +105,67 @@ def test_time_embedding_projections_as_one_group(monkeypatch, tiny, lora_rows):
         _close(out[:, G.offs[i]:G.offs[i + 1]], lora_linear_ref(sd, name, st, net.scale, lora_rows), name)
 
 
-def test_frozen_weight_copies_equal_the_state_dict(tiny):
-    """Every Linear / 1x1 weight the plans read (K-blocked or stacked) is the state-dict tensor in bf16."""
+def test_forward_operands_equal_the_state_dict(tiny):
+    """Every forward operand the plans read (K-blocked, single or stacked) is the state-dict tensors of its
+    member layers in bf16, OHWI for convolutions, each member at its first row."""
     from gemm_interp import b_matrix
     from pcm_b200 import ops
     net, sd = tiny
     checked = 0
-    for name, L in net.layers.items():
-        if L.kind in ("gn", "ln") or L.w_fwd is None or L.kind == "conv" and L.k == 3:
-            continue
-        W = sd[name + ".weight"].reshape(L.cout, -1).to(BF16)
-        assert torch.equal(b_matrix(ops.bsrc(L.w_fwd)), W), name
-        checked += 1
-    for lead, G in net.groups.items():
-        Wg = torch.cat([sd[n + ".weight"] for n in G.names], 0).to(BF16)
-        assert torch.equal(b_matrix(ops.bsrc(G.w_stack)), Wg), lead
+    for key, op in net.operands.items():
+        rows = [sd[L.name + ".weight"] for L, _ in op.members]
+        Wg = torch.cat([W.permute(0, 2, 3, 1).reshape(W.shape[0], -1) if W.dim() == 4 else W for W in rows]).to(BF16)
+        assert torch.equal(b_matrix(ops.bsrc(op.w)), Wg), key
+        assert [n0 for _, n0 in op.members] == [sum(W.shape[0] for W in rows[:i]) for i in range(len(rows))], key
         checked += 1
     assert checked > 40
+
+
+@pytest.mark.parametrize("cfg_name", ["TINY", "TINY_XL"])
+def test_each_frozen_weight_is_held_by_one_forward_operand(cfg_name):
+    """Every frozen Linear / conv weight of the layer table is held by exactly one forward operand, in a
+    storage of its own, and the operands hold exactly the table's forward-weight bytes: teacher, student and
+    target share that single copy.  No other bf16 copy of a forward weight is reachable from the layers or
+    groups (besides the dgrad operands and conv_in, whose 4-channel kernel reads its own layout)."""
+    import types
+    from pcm_b200 import config
+    from pcm_b200.unet import _Layer, _Lora
+    cfg = getattr(config, cfg_name)
+    net, _ = build_net(cfg)
+    want = {n: 2 * cout * k * k * cin if kind == "conv" else 2 * cout * cin
+            for n, kind, cin, cout, k in config.layer_table(cfg) if kind not in ("gn", "ln") and n != "conv_in"}
+    held = sorted(L.name for op in net.operands.values() for L, _ in op.members)
+    assert held == sorted(want)
+    storages = {op.w.untyped_storage().data_ptr() for op in net.operands.values()}
+    assert len(storages) == len(net.operands)
+    assert sum(op.w.untyped_storage().nbytes() for op in net.operands.values()) == sum(want.values())
+
+    def reach(obj, path, out):
+        if isinstance(obj, torch.Tensor):
+            if obj.dtype == BF16:
+                out.append((path, obj))
+        elif isinstance(obj, (list, tuple)):
+            for i, v in enumerate(obj):
+                reach(v, f"{path}[{i}]", out)
+        elif isinstance(obj, dict):
+            for k, v in obj.items():
+                reach(v, f"{path}[{k!r}]", out)
+        elif isinstance(obj, (_Layer, _Lora)):
+            for s in type(obj).__slots__:
+                reach(getattr(obj, s, None), f"{path}.{s}", out)
+        elif isinstance(obj, types.SimpleNamespace):
+            for k, v in vars(obj).items():
+                if k not in ("layers", "blocks"):           # reached through net.layers / net.groups
+                    reach(v, f"{path}.{k}", out)
+        return out
+
+    tensors = reach([net.layers, net.groups, net.temb_group, net.ctx_group], "net", [])
+    assert any(p.endswith(".w_t_cat") for p, _ in tensors) and any(".lora." in p for p, _ in tensors)
+    allowed = storages | {net.lora_opnd.untyped_storage().data_ptr()}
+    for path, t in tensors:
+        if path.rsplit(".", 1)[-1] in ("w_t", "w_t_cat", "w_c4", "w_c4_t"):
+            continue
+        assert t.untyped_storage().data_ptr() in allowed, path
 
 
 def _autograd_ref(sd, names, x, dys, scale, lora_rows):

@@ -55,16 +55,25 @@ def test_k_programs_are_valid(dry_step):
     assert ranged > 0                    # the q/k/v and cross-attention k/v groups use them
 
 
-def test_grouped_layers_replace_single_launches(dry_step):
+def test_grouped_layers_read_one_stacked_operand(dry_step):
     st, rec = dry_step
     net = st.unet
     assert net.groups
+    # the one forward operand that holds each layer, and the layer's first row in it
+    owner = {L.name: (key, op, n0) for key, op in net.operands.items() for L, n0 in op.members}
     for lead, G in net.groups.items():
         assert G.g in (2, 3)
-        # stacked frozen weights, stored K-blocked [K/64][N][64] (pcm_bsrc.kblocked)
-        assert G.w_stack.shape == (G.cin // 64, G.g * G.cout, 64)
+        # stacked frozen weights, stored K-blocked [K/64][N][64] (pcm_bsrc.kblocked): q / k / v as their own
+        # operand, cross-attention k / v as consecutive rows of a context chunk
+        key, op, n0 = owner[lead]
+        if lead.endswith(".attn1.to_q"):
+            assert key == lead and op.w.shape == (G.cin // 64, G.g * G.cout, 64)
+        else:
+            c, j = net.ctx_group.where[lead[:-len(".attn2.to_k")]]
+            ch = net.ctx_group.chunks[c]
+            assert key == ch.key and op.w.shape == (G.cin // 64, ch.n_total, 64) and n0 == 2 * j * G.cout
         for i, L in enumerate(G.layers):
-            assert L.w_fwd is None       # members are only reachable through the stacked operand
+            assert owner[L.name][0] == key and owner[L.name][2] == n0 + i * G.cout
         if G.lora:
             r = net.r
             assert G.a_stack.shape == (G.g * r, G.cin)

@@ -45,7 +45,7 @@ def test_timesteps_and_coefficients_match_the_reference_scheduler():
 
 
 @pytest.mark.parametrize("rank", [8, 64, 136, 256])
-def test_fuse_table_writes_every_lora_operand_element_once(monkeypatch, rank):
+def test_fuse_table_writes_every_fused_operand_element_once(monkeypatch, rank):
     from pcm_b200 import config
     cfg = dataclasses.replace(config.TINY_XL, lora_rank=rank)
     net, _ = build_net(cfg)
@@ -64,22 +64,29 @@ def test_fuse_table_writes_every_lora_operand_element_once(monkeypatch, rank):
     # the interpreted kernel writes every element (NaN sentinels) and leaves the sources alone
     sampler_interp.install(monkeypatch)
     inf.fused_weights.fill_(float("nan"))
-    srcs = [t.clone() for t in (net.temb_group.w_stack, *[ch.w_stack for ch in net.ctx_group.chunks])]
+    srcs = [op.w.clone() for op in net.operands.values()]
     from pcm_b200 import ops
     ops.lora_fuse(net.lora_master, table, work, net.scale)
     assert not inf.fused_weights.float().isnan().any()
-    assert all(torch.equal(a, b) for a, b in zip(srcs, (net.temb_group.w_stack,
-                                                       *[ch.w_stack for ch in net.ctx_group.chunks])))
+    assert all(torch.equal(a, op.w) for a, op in zip(srcs, net.operands.values()))
+    # the inference network shares the trained one's layers and groups; its LoRA operands are the fused copies
+    assert inf.layers is net.layers and inf.groups is net.groups and inf.ctx_group is net.ctx_group
+    base_end = base + 2 * inf.fused_weights.numel()
+    for key, op in inf.operands.items():
+        in_fused = base <= op.w.data_ptr() < base_end
+        assert in_fused == (op.members[0][0].lora is not None), key
+        assert in_fused or op.w is net.operands[key].w
     # every fused operand is W + s B A of its layers (one Linear, one conv, one stack member)
     from gemm_interp import b_matrix
     from pcm_b200 import ops as O
     for name in ("down_blocks.1.attentions.0.proj_in", "down_blocks.0.resnets.0.conv1"):
-        L, L2 = net.layers[name], inf.layers[name]
+        L = net.layers[name]
         taps = L.k * L.k if L.kind == "conv" else 1
         A = net.lora_master[L.lora.a_off:L.lora.a_off + rank * taps * L.cin].view(rank, -1)
         Bm = net.lora_master[L.lora.b_off:L.lora.b_off + L.cout * rank].view(L.cout, rank)
-        want = (b_matrix(O.bsrc(L.w_fwd)).float() + net.scale * (Bm.double() @ A.double()).float()).to(BF16)
-        assert torch.equal(b_matrix(O.bsrc(L2.w_fwd)), want)
+        W = b_matrix(O.bsrc(net.operands[name].w))
+        want = (W.float() + net.scale * (Bm.double() @ A.double()).float()).to(BF16)
+        assert torch.equal(b_matrix(O.bsrc(inf.operands[name].w)), want)
 
 
 def _inputs(ocfg, P, hw, seed=5):

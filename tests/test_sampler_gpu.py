@@ -25,20 +25,21 @@ def _unblock(w):
 
 
 @pytest.mark.parametrize("rank", [8, 64, 136, 256])
-def test_lora_fuse_matches_float64(cuda, rank):
+def test_lora_fuse_into_the_operand_list_matches_float64(cuda, rank):
     from pcm_b200 import config, ops, weights
     from pcm_b200.unet import UNetB200
     cfg = dataclasses.replace(config.TINY_XL, lora_rank=rank)
     sd = weights.synthetic_state_dict(cfg, 1, lora_b_std=0.5)
     net = UNetB200(cfg, sd, cuda, need_backward=False)
     inf, table, work = net.fused_inference_net()
-    before = [t.clone() for t in (net.temb_group.w_stack, net.ctx_group.chunks[0].w_stack)]
+    chunk = net.ctx_group.chunks[0].key
+    before = [net.operands[k].w.clone() for k in ("temb", chunk)]
     ops.lora_fuse(net.lora_master, table, work, net.scale)
     first = inf.fused_weights.clone()
     ops.lora_fuse(net.lora_master, table, work, net.scale)
     torch.cuda.synchronize()
     assert torch.equal(first, inf.fused_weights)          # repeats are bitwise equal
-    assert all(torch.equal(a, b) for a, b in zip(before, (net.temb_group.w_stack, net.ctx_group.chunks[0].w_stack)))
+    assert all(torch.equal(a, net.operands[k].w) for a, k in zip(before, ("temb", chunk)))
     s = net.scale
 
     def want(name):
@@ -69,15 +70,14 @@ def test_lora_fuse_matches_float64(cuda, rank):
         assert (got != exp.to(BF).double()).double().mean().item() < 0.01        # < 1 % off the nearest
 
     lin = "down_blocks.1.attentions.0.transformer_blocks.0.attn1.to_out.0"
-    check(_unblock(inf.layers[lin].w_fwd), *want(lin))
+    check(_unblock(inf.operands[lin].w), *want(lin))
     conv = "down_blocks.1.resnets.0.conv1"
-    check(_unblock(inf.layers[conv].w_fwd), *want(conv))
+    check(_unblock(inf.operands[conv].w), *want(conv))
     lead = "down_blocks.1.attentions.0.transformer_blocks.0.attn1.to_q"
-    check(_unblock(inf.groups[lead].w_stack), *stacked([lead[:-1] + c for c in "qkv"]))
-    check(_unblock(inf.temb_group.w_stack), *stacked(inf.temb_group.names))
-    ch = inf.ctx_group.chunks[0]
+    check(_unblock(inf.operands[lead].w), *stacked([lead[:-1] + c for c in "qkv"]))
+    check(_unblock(inf.operands["temb"].w), *stacked(inf.temb_group.names))
     names = [n for G in net.ctx_group.chunks[0].blocks for n in G.names]
-    check(_unblock(ch.w_stack), *stacked(names))
+    check(_unblock(inf.operands[chunk].w), *stacked(names))
 
 
 @pytest.mark.parametrize("pred", [0, 1])
