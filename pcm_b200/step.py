@@ -146,7 +146,7 @@ class PCMTrainStep:
         eps_all = u.forward(self.noisy3[:nb * B], self.start_t3[:nb * B],
                             self.in_ctx3 if nb == 3 else self.in_ctx3[:2 * B * 77],
                             lora=True, save=True, lora_batch=B, added_cond=added(0, nb * B))
-        kv = u.last_ctx_kv
+        kv = u.saved_ctx_kv()
         eps_s, eps_c = eps_all[:B], eps_all[B:2 * B]
         eps_u = eps_all[2 * B:] if nb == 3 else eps_c
         # the target network is the student (same LoRA factors) on the same prompt embeddings

@@ -13,10 +13,11 @@ teacher, :1263-1268 target) and its autograd backward (:1296), with:
 Parameters use diffusers state-dict names; LoRA factors live in ONE flat fp32 buffer
 (`lora_master`), their gradients in `lora_grad`.
 """
+import copy
 import types
 import weakref
 from collections import namedtuple
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Optional
 
 import torch
@@ -133,9 +134,57 @@ def _stacks(tab):
     return out + [(f"ctx.{c}", "ctx", ch) for c, ch in enumerate(chunks)]
 
 
+@dataclass
+class _Pass:
+    """One forward pass: what its primitives read besides their own arguments."""
+    lora: bool                              # the LoRA adapters are on
+    B: int                                  # samples in the batch
+    lb: int                                 # the leading samples that carry the adapter
+    plan_b: Optional[int] = None            # a rebuilt block: the merged pass's batch, whose plans it keeps
+    st: Optional[torch.Tensor] = None       # silu(temb) [B, C]
+    ctx: Optional[torch.Tensor] = None      # text context [B*S, D]
+    temb: Optional[tuple] = None            # UNetB200.temb_all: (out_all, T)
+    ctxkv: Optional[dict] = None            # UNetB200.ctx_kv_all: {transformer block: (k, v, T)}
+
+    def rows(self, n):
+        """Rows / samples of an n-row (batch-major) tensor that belong to the LoRA samples."""
+        return n * self.lb // self.B
+
+    def tiling(self, M, N, prog):
+        """Tiling keywords of a block's main GEMM.  Empty (ops.gemm picks from M) except in a rebuilt
+        block: then the (block_n, ksplit) the merged pass picked for its larger M, since pick_tiling splits
+        K by M and the split decides how the fp32 sums round.  The LoRA down-projections already ran on the
+        student rows alone and need nothing."""
+        if self.plan_b is None:
+            return {}
+        bn, ks = ops.pick_tiling(M * self.plan_b // self.B, N, sum(e[4] for e in prog))
+        return dict(block_n=bn, ksplit=ks)
+
+    def student(self):
+        """The pass a checkpointed block of this one is rebuilt in: the student rows of its time embedding,
+        context, grouped time_emb_proj output and context k / v, with this pass's launch plans."""
+        lb, S = self.lb, self.ctx.shape[0] // self.B
+        kv = self.ctxkv and {t: (k[:lb * S], v[:lb * S], T) for t, (k, v, T) in self.ctxkv.items()}
+        return _Pass(self.lora, lb, lb, self.B if self.B != lb else None, self.st[:lb], self.ctx[:lb * S],
+                     (self.temb[0][:lb], self.temb[1]), kv)
+
+
+# forward(save=True) for backward(): the block records in forward order, the head GroupNorm's record,
+# (student samples, H, W) and the student pass that rebuilds checkpointed blocks (None: no checkpointing)
+Saved = namedtuple("Saved", "tape head shape rebuild")
+
+
+@dataclass
+class _Backward:
+    """Scratch of one backward() call."""
+    wstream: Optional[torch.cuda.Stream] = None  # the weight-gradient side stream (None: none, all in order)
+    dkv: dict = field(default_factory=dict)     # per context chunk: the dk / dv matrix of its shape
+    keep: list = field(default_factory=list)    # tensors the weight-gradient stream reads (_Side)
+    side: list = field(default_factory=list)    # checkpointing: (event, keep) of the last blocks walked
+
+
 class UNetB200:
     gradient_checkpointing = False
-    _plan_b = None
 
     def __init__(self, cfg: UNetConfig, state_dict, device, need_backward=True, lora=True,
                  gradient_checkpointing=False):
@@ -248,18 +297,10 @@ class UNetB200:
         self._build_temb_group(next(names for _, kind, names in stacks if kind == "temb"))
         self._build_ctx_group([(key, names) for key, kind, names in stacks if kind == "ctx"])
         self.saved = None
-        self._temb = None
-        self._ctxkv = self.last_ctx_kv = None
-        self._dkv_chunks = {}
-        self._lb = (1, 1)
-        # while backward() rebuilds a checkpointed block: the batch of the merged pass that first ran it,
-        # whose launch plans the rebuild keeps (_merged_tiling, gn)
-        self._plan_b = None
         # LoRA weight-gradient GEMMs are off the dgrad critical path (they only feed the optimiser):
         # they run on a side stream and fill SMs the main backward chain leaves idle
-        self.use_wstream = torch.device(device).type == "cuda" and need_backward and lora
-        self.wstream = torch.cuda.Stream(device=device) if self.use_wstream else None
-        self._keep = []
+        use_wstream = torch.device(device).type == "cuda" and need_backward and lora
+        self.wstream = torch.cuda.Stream(device=device) if use_wstream else None
 
     def _kblocked(self, W):
         """bf16 copy of the fp32 [N, K] matrix W on the device, K-blocked [K/64][N][64] (pcm_bsrc.kblocked):
@@ -358,12 +399,12 @@ class UNetB200:
                  dep_a_src=dep_a_src)
         return out
 
-    def temb_all(self, st, lora):
-        """All time_emb_proj layers of one pass: out[B, sum C_i] = [st | T] @ [W ; N-ranged s*B_i]^T + b.
+    def temb_all(self, P):
+        """All time_emb_proj layers of pass P: out[B, sum C_i] = [st | T] @ [W ; N-ranged s*B_i]^T + b.
         Returns (out, T): resnet i uses the column view out[:, offs[i]:offs[i+1]] as its row vector and
         column block i of T for its LoRA weight gradients."""
-        G, r = self.temb_group, self.r
-        T = self._lora_down(st[:self._lrows(st.shape[0])], G.a_stack) if lora and G.lora else None
+        G, r, st = self.temb_group, self.r, P.st
+        T = self._lora_down(st[:P.rows(st.shape[0])], G.a_stack) if P.lora and G.lora else None
         out = self._stacked_gemm(st, self.operands["temb"].w, T, getattr(G, "sb_stack", None),
                                  [(i * r, G.offs[i], G.offs[i + 1]) for i in range(G.g)], G.n_total,
                                  block_n=G.bn, bias=G.bias)
@@ -398,11 +439,11 @@ class UNetB200:
             first += len(ch_names)
         self.ctx_group = CG
 
-    def ctx_kv_all(self, ctx, lora):
-        """{transformer block: (k, v, T)} for one pass: k / v are column views [M, C] of the chunk outputs,
+    def ctx_kv_all(self, P):
+        """{transformer block: (k, v, T)} for pass P: k / v are column views [M, C] of the chunk outputs,
         T the block's two columns blocks [Ml, 2r] of the stacked LoRA down-projection (None without LoRA)."""
-        CG, r = self.ctx_group, self.r
-        T = self._lora_down(ctx[:self._lrows(ctx.shape[0])], CG.a_stack) if lora and CG.lora else None
+        CG, r, ctx = self.ctx_group, self.r, P.ctx
+        T = self._lora_down(ctx[:P.rows(ctx.shape[0])], CG.a_stack) if P.lora and CG.lora else None
         outs = [self._stacked_gemm(ctx, self.operands[ch.key].w, T, getattr(ch, "sb_stack", None),
                                    [((ch.first + i) * r, i * ch.cout, (i + 1) * ch.cout)
                                     for i in range(2 * len(ch.blocks))], ch.n_total, block_n=ch.bn)
@@ -423,20 +464,20 @@ class UNetB200:
 
     class _Side:
         """Run the enclosed launches on the wgrad side stream, ordered after everything enqueued so far
-        on the current stream; `keep` tensors stay referenced until backward() joins the streams."""
+        on the current stream; `keep` tensors stay referenced (bw.keep) until backward() joins the streams."""
 
-        def __init__(self, net, keep):
-            self.net, self.keep, self.ctx = net, keep, None
+        def __init__(self, bw, keep):
+            self.bw, self.keep, self.ctx = bw, keep, None
 
         def __enter__(self):
-            n = self.net
-            if not n.use_wstream:
+            bw = self.bw
+            if bw.wstream is None:
                 return self
             ev = torch.cuda.Event()
             ev.record()
-            n.wstream.wait_event(ev)
-            n._keep.extend(self.keep)
-            self.ctx = torch.cuda.stream(n.wstream)
+            bw.wstream.wait_event(ev)
+            bw.keep.extend(self.keep)
+            self.ctx = torch.cuda.stream(bw.wstream)
             self.ctx.__enter__()
             return self
 
@@ -444,11 +485,6 @@ class UNetB200:
             if self.ctx is not None:
                 self.ctx.__exit__(*a)
             return False
-
-    def _join_side(self):
-        if self.use_wstream:
-            torch.cuda.current_stream().wait_stream(self.wstream)
-            self._keep.clear()
 
     # ------------------------------------------------------------------------------------
     def refresh_lora(self, master=None):
@@ -470,15 +506,11 @@ class UNetB200:
         n, work_begin}."""
         if not self.has_lora:
             raise ValueError("fused_inference_net needs a network built with lora=True")
-        net = object.__new__(UNetB200)
-        net.__dict__.update(self.__dict__)
+        net = copy.copy(self)
         for k in ("lora_master", "lora_grad", "lora_opnd", "refresh_table", "refresh_work"):
             net.__dict__.pop(k, None)
-        net.has_lora, net.use_wstream, net.wstream = False, False, None
-        net.gradient_checkpointing = False
-        net.lora_layers, net._keep, net._dkv_chunks = [], [], {}
-        net.saved = net._temb = net._ctxkv = net.last_ctx_kv = None
-        net._lb, net._plan_b = (1, 1), None
+        net.has_lora, net.wstream = False, None
+        net.gradient_checkpointing, net.lora_layers, net.saved = False, [], None
         fused = {key: op for key, op in self.operands.items() if any(L.lora is not None for L, _ in op.members)}
         net.fused_weights = torch.empty(sum(op.w.numel() for op in fused.values()), device=self.dev, dtype=BF16)
         net.operands = dict(self.operands)
@@ -572,17 +604,7 @@ class UNetB200:
             coff += ci
         return srcs, prog
 
-    def _merged_tiling(self, M, N, prog):
-        """Tiling keywords of a block's main GEMM.  Empty (ops.gemm picks from M) except while backward()
-        rebuilds a checkpointed block: then the (block_n, ksplit) the merged pass picked for its larger M,
-        since pick_tiling splits K by M and the split decides how the fp32 sums round.  The LoRA
-        down-projections already ran on the student rows alone and need nothing."""
-        if self._plan_b is None:
-            return {}
-        bn, ks = ops.pick_tiling(M * self._plan_b // self._lb[1], N, sum(e[4] for e in prog))
-        return dict(block_n=bn, ksplit=ks)
-
-    def conv3(self, name, xs, lora, stride=1, rowvec=None, residual=None, out_fp32=False, save=None):
+    def conv3(self, P, name, xs, stride=1, rowvec=None, residual=None, out_fp32=False, save=None):
         """3x3 pad-1 convolution (+LoRA) over NHWC sources xs (channel concat), fused epilogue; appends its
         ConvRec to the list `save`."""
         L = self.layers[name]
@@ -592,9 +614,9 @@ class UNetB200:
         srcs, prog = self._conv_prog(xs, 3, stride, L.cin)
         bs = [ops.bsrc(self.operands[name].w)]
         T = None
-        lbn = self._lrows(B)   # samples that carry the LoRA adapter (the leading ones of the batch)
+        lbn = P.rows(B)   # samples that carry the LoRA adapter (the leading ones of the batch)
         xl = xs if lbn == B else [x[:lbn] for x in xs]
-        if lora and L.lora is not None:
+        if P.lora and L.lora is not None:
             # T = A(x) only for the LoRA samples; the other samples see T rows that TMA zero-fills
             T = self._new(lbn, Ho, Wo, self.r)
             srcs_l, prog_l = (srcs, prog) if lbn == B else self._conv_prog(xl, 3, stride, L.cin)
@@ -607,12 +629,12 @@ class UNetB200:
         ops.gemm(srcs, bs, prog, lin=False, M=M, N=N, geo=(Wo, Ho), out=out.view(M, N), bias=L.bias,
                  rowvec=rowvec, residual=None if residual is None else residual.reshape(M, N),
                  round_bf16=out_fp32, dep_a_src=None if T is None else len(srcs) - 1,
-                 **self._merged_tiling(M, N, prog))
+                 **P.tiling(M, N, prog))
         if save is not None:
             save.append(ConvRec("conv3", name, xl, T, stride))
         return out
 
-    def linear(self, name, xs, lora, residual=None, act=0, save=None):
+    def linear(self, P, name, xs, residual=None, act=0, save=None):
         """nn.Linear / 1x1 conv over [M, C] matrices xs (channel concat) (+LoRA), fused epilogue; appends its
         LinearRec to the list `save`."""
         L = self.layers[name]
@@ -624,9 +646,9 @@ class UNetB200:
             coff += x.shape[1]
         bs = [ops.bsrc(self.operands[name].w)]
         T = None
-        Ml = self._lrows(M)
+        Ml = P.rows(M)
         xl = xs if Ml == M else [x[:Ml] for x in xs]
-        if lora and L.lora is not None:
+        if P.lora and L.lora is not None:
             T = self._new(Ml, self.r)
             srcs_l = srcs if Ml == M else [ops.asrc_mat(x) for x in xl]
             ops.gemm(srcs_l, [ops.bsrc(L.lora.a_fwd)], prog, lin=True, M=Ml, N=self.r, out=T)
@@ -635,20 +657,20 @@ class UNetB200:
             bs.append(ops.bsrc(L.lora.sb_fwd))
         out = self._new(M, N)
         ops.gemm(srcs, bs, prog, lin=True, M=M, N=N, out=out, bias=L.bias, residual=residual, act=act,
-                 dep_a_src=None if T is None else len(srcs) - 1, **self._merged_tiling(M, N, prog))
+                 dep_a_src=None if T is None else len(srcs) - 1, **P.tiling(M, N, prog))
         if save is not None:
             save.append(LinearRec("linear", name, xl, T))
         return out
 
-    def linear_group(self, lead, x, lora, save=None):
+    def linear_group(self, P, lead, x, save=None):
         """The g Linear layers of a shared-input group (attn1 q/k/v, attn2 k/v) as ONE GEMM:
         out[M, g*C] = x @ [W_0; ...; W_g-1]^T, layer i's LoRA up-projection entering as a K block that
         only feeds its own C output columns.  Returns the g column views of out; appends its GroupRec to
         the list `save`."""
         G, r = self.groups[lead], self.r
         g, Cc = G.g, G.cout
-        xl = x[:self._lrows(x.shape[0])]
-        T = self._lora_down(xl, G.a_stack) if lora and G.lora else None
+        xl = x[:P.rows(x.shape[0])]
+        T = self._lora_down(xl, G.a_stack) if P.lora and G.lora else None
         out = self._stacked_gemm(x, self.operands[lead].w, T, getattr(G, "sb_stack", None),
                                  [(i * r, i * Cc, (i + 1) * Cc) for i in range(g)], g * Cc,
                                  block_n=160 if Cc % 160 == 0 else 64, dep_a_src=None if T is None else 1)
@@ -656,39 +678,39 @@ class UNetB200:
             save.append(GroupRec("lgroup", lead, xl, T))
         return [out[:, i * Cc:(i + 1) * Cc] for i in range(g)]
 
-    def gn(self, name, xs, B, HW, eps, silu, save=None):
+    def gn(self, P, name, xs, B, HW, eps, silu, save=None):
         L = self.layers[name]
         C = sum(x.shape[-1] for x in xs)
         out = self._new(B * HW, C)
         stats = self._new(B, self.cfg.norm_num_groups, 2, dtype=torch.float32)
         x2 = xs[1] if len(xs) > 1 else None
-        if self._plan_b is None:
+        if P.plan_b is None:
             ops.groupnorm_fwd(xs[0], x2, L.gamma, L.beta, eps, silu, out, stats, B, HW, self.cfg.norm_num_groups)
         else:   # a rebuilt block: merge each image's statistics from the merged pass's partition
-            ops.groupnorm_fwd_part(xs[0], x2, L.gamma, L.beta, eps, silu, out, stats, B, self._plan_b, HW,
+            ops.groupnorm_fwd_part(xs[0], x2, L.gamma, L.beta, eps, silu, out, stats, B, P.plan_b, HW,
                                    self.cfg.norm_num_groups)
         if save is not None:
-            lb = self._lrows(B)
+            lb = P.rows(B)
             save.append(GNRec("gn", name, xs if lb == B else [x[:lb * HW] for x in xs], stats[:lb], eps, silu, lb, HW))
         return out
 
-    def ln(self, name, x, save=None):
+    def ln(self, P, name, x, save=None):
         L = self.layers[name]
         out = torch.empty_like(x)
         stats = self._new(x.shape[0], 2, dtype=torch.float32)
         ops.layernorm_fwd(x, L.gamma, L.beta, out, stats)
         if save is not None:
-            Ml = self._lrows(x.shape[0])
+            Ml = P.rows(x.shape[0])
             save.append(LNRec("ln", name, x[:Ml], stats[:Ml]))
         return out
 
-    def attention(self, q, k, v, B, Sq, Skv, heads, save=None):
+    def attention(self, P, q, k, v, B, Sq, Skv, heads, save=None):
         D = q.shape[1] // heads
         out = self._new(q.shape[0], q.shape[1])
         lse = self._new(B, heads, Sq, dtype=torch.float32)
         ops.attn_fwd(q, k, v, out, lse, B, heads, Sq, Skv, D, D ** -0.5)
         if save is not None:
-            lb = self._lrows(B)
+            lb = P.rows(B)
             save.append(AttnRec("attn", q[:lb * Sq], k[:lb * Skv], v[:lb * Skv], out[:lb * Sq], lse[:lb], lb, Sq, Skv,
                                 heads))
         return out
@@ -696,7 +718,7 @@ class UNetB200:
     # ------------------------------------------------------------------------------------
     # blocks (forward): each returns (out, block record)
     # ------------------------------------------------------------------------------------
-    def resnet(self, p, xs, st, lora, save):
+    def resnet(self, P, p, xs, save):
         """xs: list of NHWC sources (skip concat = 2 sources).  Returns ([B,H,W,Cout], ResnetRec)."""
         B, H, W, _ = xs[0].shape
         HW = H * W
@@ -704,23 +726,23 @@ class UNetB200:
         cout = self.layers[p + ".conv1"].cout
         flat = [x.view(B * HW, x.shape[-1]) for x in xs]
         s = [] if save else None        # this block's op records
-        h = self.gn(p + ".norm1", flat, B, HW, 1e-5, True, s)
+        h = self.gn(P, p + ".norm1", flat, B, HW, 1e-5, True, s)
         norm1 = _last(s)
         G = self.temb_group
         i = G.index[p + ".time_emb_proj"]
-        out_all, T_all = self._temb
+        out_all, T_all = P.temb
         # the grouped launch of temb_all computed this layer: its record only names the column block
-        temb = TembRec("linear", p + ".time_emb_proj", [st[:self._lrows(st.shape[0])]], T_all, i * self.r)
-        h = self.conv3(p + ".conv1", [h.view(B, H, W, cin)], lora, rowvec=out_all[:, G.offs[i]:G.offs[i + 1]],
+        temb = TembRec("linear", p + ".time_emb_proj", [P.st[:P.rows(P.st.shape[0])]], T_all, i * self.r)
+        h = self.conv3(P, p + ".conv1", [h.view(B, H, W, cin)], rowvec=out_all[:, G.offs[i]:G.offs[i + 1]],
                        save=s)
         conv1 = _last(s)
-        h = self.gn(p + ".norm2", [h.view(B * HW, cout)], B, HW, 1e-5, True, s)
+        h = self.gn(P, p + ".norm2", [h.view(B * HW, cout)], B, HW, 1e-5, True, s)
         norm2 = _last(s)
         sc, shortcut = xs[0], None
         if cin != cout:
-            sc = self.linear(p + ".conv_shortcut", flat, lora, save=s).view(B, H, W, cout)
+            sc = self.linear(P, p + ".conv_shortcut", flat, save=s).view(B, H, W, cout)
             shortcut = _last(s)
-        out = self.conv3(p + ".conv2", [h.view(B, H, W, cout)], lora, residual=sc, save=s)
+        out = self.conv3(P, p + ".conv2", [h.view(B, H, W, cout)], residual=sc, save=s)
         return out, ResnetRec(p, norm1, temb, conv1, norm2, shortcut, _last(s), takes_skip=len(xs) == 2)
 
     def _level_of(self, name):
@@ -732,7 +754,7 @@ class UNetB200:
         i = int(parts[1])
         return i if parts[0] == "down_blocks" else nb - 1 - i
 
-    def transformer(self, p, x, ctx, lora, save):
+    def transformer(self, P, p, x, save):
         """Transformer2DModel: GN -> proj_in -> depth x BasicTransformerBlock -> proj_out -> + residual.
         proj_in / proj_out are 1x1 convolutions (SD1.5) or nn.Linear (SDXL, use_linear_projection):
         on NHWC tokens both are the same GEMM."""
@@ -742,60 +764,55 @@ class UNetB200:
         heads = self.cfg.heads(level)
         xf = x.view(M, C)
         s = [] if save else None        # this block's op records
-        g = self.gn(p + ".norm", [xf], B, S, 1e-6, False, s)
+        g = self.gn(P, p + ".norm", [xf], B, S, 1e-6, False, s)
         norm = _last(s)
-        h = self.linear(p + ".proj_in", [g], lora, save=s)
+        h = self.linear(P, p + ".proj_in", [g], save=s)
         proj_in = _last(s)
         blocks = []
         for d in range(self.cfg.depth(level)):
             t = p + f".transformer_blocks.{d}"
             b = [] if save else None    # the op records of one transformer block, in TBlockRec order
-            n = self.ln(t + ".norm1", h, b)
-            q, k, v = self.linear_group(t + ".attn1.to_q", n, lora, save=b)
-            a = self.attention(q, k, v, B, S, S, heads, b)
-            h = self.linear(t + ".attn1.to_out.0", [a], lora, residual=h, save=b)
-            n = self.ln(t + ".norm2", h, b)
-            q = self.linear(t + ".attn2.to_q", [n], lora, save=b)
-            k, v, Tkv = self._ctxkv[t]
+            n = self.ln(P, t + ".norm1", h, b)
+            q, k, v = self.linear_group(P, t + ".attn1.to_q", n, save=b)
+            a = self.attention(P, q, k, v, B, S, S, heads, b)
+            h = self.linear(P, t + ".attn1.to_out.0", [a], residual=h, save=b)
+            n = self.ln(P, t + ".norm2", h, b)
+            q = self.linear(P, t + ".attn2.to_q", [n], save=b)
+            k, v, Tkv = P.ctxkv[t]
             if save:    # k / v came from the context chunks of ctx_kv_all; Tkv is this block's window of T
-                b.append(GroupRec("lgroup", t + ".attn2.to_k", ctx[:self._lrows(ctx.shape[0])], Tkv))
-            a = self.attention(q, k, v, B, S, ctx.shape[0] // B, heads, b)
-            h = self.linear(t + ".attn2.to_out.0", [a], lora, residual=h, save=b)
-            n = self.ln(t + ".norm3", h, b)
-            u = self.linear(t + ".ff.net.0.proj", [n], lora, save=b)
+                b.append(GroupRec("lgroup", t + ".attn2.to_k", P.ctx[:P.rows(P.ctx.shape[0])], Tkv))
+            a = self.attention(P, q, k, v, B, S, P.ctx.shape[0] // B, heads, b)
+            h = self.linear(P, t + ".attn2.to_out.0", [a], residual=h, save=b)
+            n = self.ln(P, t + ".norm3", h, b)
+            u = self.linear(P, t + ".ff.net.0.proj", [n], save=b)
             gg = self._new(M, u.shape[1] // 2)
             ops.geglu_fwd(u, gg)
             if save:
-                b.append(GegluRec("geglu", u[:self._lrows(M)]))
-            h = self.linear(t + ".ff.net.2", [gg], lora, residual=h, save=b)
+                b.append(GegluRec("geglu", u[:P.rows(M)]))
+            h = self.linear(P, t + ".ff.net.2", [gg], residual=h, save=b)
             blocks.append(TBlockRec._make(b) if save else None)
-        out = self.linear(p + ".proj_out", [h], lora, residual=xf, save=s)
+        out = self.linear(P, p + ".proj_out", [h], residual=xf, save=s)
         return out.view(B, H, W, C), TransformerRec(p, norm, proj_in, blocks, _last(s))
 
-    def resample(self, name, x, lora, save, up):
+    def resample(self, P, name, x, save, up):
         """Downsampler (stride-2 convolution) or upsampler (nearest 2x, then the convolution)."""
         s = [] if save else None
         if not up:
-            out = self.conv3(name, [x], lora, stride=2, save=s)
+            out = self.conv3(P, name, [x], stride=2, save=s)
         else:
             B, H, W, C = x.shape
             xu = self._new(B, 2 * H, 2 * W, C)
             ops.upsample2x_fwd(x, xu)
-            out = self.conv3(name, [xu], lora, save=s)
+            out = self.conv3(P, name, [xu], save=s)
         return out, ResampleRec(name, _last(s), up)
 
-    def _block(self, kind, name, xs, st, ctx, lora, save, up=False):
-        """One block's forward: (out, record)."""
+    def _block(self, kind, name, xs, P, save, up=False):
+        """One block's forward in pass P: (out, record)."""
         if kind == "resnet":
-            return self.resnet(name, xs, st, lora, save)
+            return self.resnet(P, name, xs, save)
         if kind == "transformer":
-            return self.transformer(name, xs[0], ctx, lora, save)
-        return self.resample(name, xs[0], lora, save, up)
-
-    def _lrows(self, n):
-        """Rows / samples of an n-row (batch-major) tensor that belong to the LoRA samples."""
-        lb, bt = self._lb
-        return n * lb // bt
+            return self.transformer(P, name, xs[0], save)
+        return self.resample(P, name, xs[0], save, up)
 
     def forward(self, sample, timesteps, ctx, lora=True, save=False, lora_batch=None, added_cond=None,
                 ctx_kv=None):
@@ -812,46 +829,46 @@ class UNetB200:
         With gradient_checkpointing, save=True keeps a CheckpointRec per block instead: owned copies of
         the student rows of the block's inputs (one copy per tensor: a down-path output that is the next
         block's input and a skip is kept once), so the merged pass's activations and every block-internal
-        tensor are freed as the forward proceeds.  The time-embedding and context projections of the pass
-        stay referenced (small), and the head's GroupNorm record keeps a copy of its student rows.
-        backward() then rebuilds one block's full record at a time."""
+        tensor are freed as the forward proceeds.  The student pass (the student rows of the pass's time-
+        embedding and context projections, small) stays referenced, and the head's GroupNorm record keeps a
+        copy of its student rows.  backward() then rebuilds one block's full record at a time."""
         cfg = self.cfg
         lora = lora and self.has_lora
         B, H, W, _ = sample.shape
-        self._lb = (lora_batch if (lora and lora_batch) else B, B)
+        P = _Pass(lora, B, lora_batch if (lora and lora_batch) else B, ctx=ctx)
         c0 = cfg.block_out_channels[0]
         emb = self._new(B, c0)
         ops.timestep_embed(timesteps, emb)
-        hemb = self.linear("time_embedding.linear_1", [emb], False, act=1)
+        # the time and added embeddings are no LoRA targets: P.lora leaves them frozen
+        hemb = self.linear(P, "time_embedding.linear_1", [emb], act=1)
         if not cfg.addition_embed:
-            st = self.linear("time_embedding.linear_2", [hemb], False, act=1)  # silu(temb)
+            P.st = self.linear(P, "time_embedding.linear_2", [hemb], act=1)  # silu(temb)
         else:
             # "text_time": emb = time_embedding(t) + add_embedding(cat[text_embeds, sinusoid(time_ids)]);
             # every consumer takes silu(emb): the sum and the SiLU run in the last GEMM's epilogue
             if added_cond is None:
                 raise ValueError("this UNet needs added_cond = (text_embeds, time_ids) (addition_embed_type text_time)")
             text_embeds, time_ids = added_cond
-            temb = self.linear("time_embedding.linear_2", [hemb], False)
+            temb = self.linear(P, "time_embedding.linear_2", [hemb])
             tid = self._new(B * cfg.num_time_ids, cfg.addition_time_embed_dim)
             ops.timestep_embed(time_ids.reshape(-1), tid)
             add_in = torch.cat([text_embeds.to(BF16), tid.view(B, -1)], dim=1).contiguous()  # [B, 2816] glue
-            ah = self.linear("add_embedding.linear_1", [add_in], False, act=1)
-            st = self.linear("add_embedding.linear_2", [ah], False, residual=temb, act=1)
-        self._temb = self.temb_all(st, lora)
+            ah = self.linear(P, "add_embedding.linear_1", [add_in], act=1)
+            P.st = self.linear(P, "add_embedding.linear_2", [ah], residual=temb, act=1)
+        P.temb = self.temb_all(P)
         # cross-attention k / v of every block: given (ctx_kv: another pass of this step already projected
         # the same context with the same weights) or computed here in a few grouped GEMMs
         if ctx_kv is not None:
             assert not save
-            self._ctxkv = ctx_kv
-        else:
-            self._ctxkv = self.ctx_kv_all(ctx, lora) if self.ctx_group is not None else None
-        self.last_ctx_kv = self._ctxkv if lora else None
+            P.ctxkv = ctx_kv
+        elif self.ctx_group is not None:
+            P.ctxkv = self.ctx_kv_all(P)
         x = self._new(B, H, W, c0)
         Lci = self.layers["conv_in"]
         ops.conv3x3_c4(sample, Lci.w_c4, Lci.bias, x, sgn=1, round_in=True)
         tape, skips = [], [x]       # tape: the block records in forward order
         ck = save and self.gradient_checkpointing
-        lb = self._lb[0]
+        lb = P.lb
         copies = {}                 # checkpointing: id of a block input -> (weak reference, its copy)
 
         def student_rows(xs):
@@ -867,8 +884,8 @@ class UNetB200:
         def run(kind, name, xs, up=False):
             if ck:
                 tape.append(CheckpointRec(kind, name, student_rows(xs), len(xs) == 2, up))
-                return self._block(kind, name, xs, st, ctx, lora, False, up)[0]
-            out, rec = self._block(kind, name, xs, st, ctx, lora, save, up)
+                return self._block(kind, name, xs, P, False, up)[0]
+            out, rec = self._block(kind, name, xs, P, save, up)
             tape.append(rec)
             return out
 
@@ -898,42 +915,23 @@ class UNetB200:
                 x = run("resample", f"up_blocks.{i}.upsamplers.0.conv", [x], up=True)
         Bx, Hx, Wx, Cx = x.shape
         head = [] if save else None
-        g = self.gn("conv_norm_out", [x.view(Bx * Hx * Wx, Cx)], Bx, Hx * Wx, 1e-5, True, head)
-        eps = self.conv3("conv_out", [g.view(Bx, Hx, Wx, Cx)], False, out_fp32=True)
+        g = self.gn(P, "conv_norm_out", [x.view(Bx * Hx * Wx, Cx)], Bx, Hx * Wx, 1e-5, True, head)
+        eps = self.conv3(P, "conv_out", [g.view(Bx, Hx, Wx, Cx)], out_fp32=True)
         if save:
-            rebuild = None
-            if ck:
-                h = head[0]      # already the student rows: views of the merged pass's last activation
-                if lb != B:
-                    head[0] = h._replace(xs=[t.clone() for t in h.xs], stats=h.stats.clone())
-                rebuild = self._rebuild_state(lora, B, st, ctx)
-            self.saved = (tape, head[0], (lb, H, W), rebuild)
+            h = head[0]
+            if ck and lb != B:      # the student rows are views of the merged pass's last activation
+                h = h._replace(xs=[t.clone() for t in h.xs], stats=h.stats.clone())
+            self.saved = Saved(tape, h, (lb, H, W), P.student() if ck else None)
         return eps
 
-    def _rebuild_state(self, lora, B, st, ctx):
-        """What rebuilding a checkpointed block of this pass needs besides its inputs: the student rows of
-        the pass's time embedding, of its grouped time_emb_proj output and of its context k / v."""
-        lb = self._lb[0]
-        out_all, T = self._temb
-        kv = self._ctxkv
-        S = ctx.shape[0] // B
-        if kv is not None:
-            kv = {t: (k[:lb * S], v[:lb * S], Tkv) for t, (k, v, Tkv) in kv.items()}
-        return types.SimpleNamespace(lora=lora, B=B, lb=lb, st=st[:lb], ctx=ctx[:lb * S], temb=(out_all[:lb], T),
-                                     ctxkv=kv)
-
-    def _rebuild(self, ck, state):
-        """The full record of a checkpointed block: its forward once more, on the saved student rows, with
-        the launch plans of the merged pass that first ran it, so that every tensor of the record is
-        bitwise the one the stored tape would hold."""
-        prev = self._lb, self._temb, self._ctxkv
-        self._lb, self._temb, self._ctxkv = (state.lb, state.lb), state.temb, state.ctxkv
-        self._plan_b = state.B if state.B != state.lb else None
-        try:
-            return self._block(ck.kind, ck.name, ck.xs, state.st, state.ctx, state.lora, True, ck.up)[1]
-        finally:
-            self._lb, self._temb, self._ctxkv = prev
-            self._plan_b = None
+    def saved_ctx_kv(self):
+        """{transformer block: (k, v, T)}: the student rows of the context k / v of the pass forward(save=True)
+        saved, which a later pass of the student on the same context takes (forward(ctx_kv=...))."""
+        tape, _, _, rebuild = self.saved
+        if rebuild is not None:
+            return rebuild.ctxkv
+        return {f"{blk.name}.transformer_blocks.{d}": (b.attn2.k, b.attn2.v, b.attn2_kv.T)
+                for blk in tape if isinstance(blk, TransformerRec) for d, b in enumerate(blk.blocks)}
 
     # ------------------------------------------------------------------------------------
     # backward primitives
@@ -956,7 +954,7 @@ class UNetB200:
                 ops.wgrad(psrc, dt, lo.gA[64 * j:], lin=lin, M=M, geo=geo, taps=taps, tap_off=offs, os_row=1,
                           os_col=lo.gA.shape[1], q_c0=dt_c0 + 64 * j)
 
-    def linear_bwd(self, rec, dy, need_dx=True, t_c0=0):
+    def linear_bwd(self, bw, rec, dy, need_dx=True, t_c0=0):
         """rec: LinearRec (or TembRec, whose block of T starts at column t_c0).  Returns dx [M, cin_total]
         (or None)."""
         L = self.layers[rec.name]
@@ -971,7 +969,7 @@ class UNetB200:
             for x in rec.xs:
                 P_list.append((ops.asrc_mat(x), ((0, 0),), (coff,)))
                 coff += x.shape[1]
-            with UNetB200._Side(self, (dy, rec.T, dt, *rec.xs)):
+            with UNetB200._Side(bw, (dy, rec.T, dt, *rec.xs)):
                 self._lora_wgrads(L, M, ops.asrc_mat(dy), ops.asrc_mat(rec.T), ops.asrc_mat(dt), P_list,
                                   t_c0=t_c0)
         if not need_dx:
@@ -986,7 +984,7 @@ class UNetB200:
         ops.gemm(srcs, bs, prog, lin=True, M=M, N=L.cin, out=dx, dep_a_src=None if dt is None else 1)
         return dx
 
-    def linear_group_bwd(self, rec, dpk, need_dx=True):
+    def linear_group_bwd(self, bw, rec, dpk, need_dx=True):
         """rec: GroupRec ("lgroup", lead, x, T); dpk [M, g*C] = the g output gradients side by side.
         Returns dx [M, cin] (or None): ONE dgrad GEMM over K = g*C (+ the g LoRA blocks)."""
         _, lead, x, T = rec
@@ -1006,7 +1004,7 @@ class UNetB200:
                 for i in range(g):
                     ops.gemm([ops.asrc_mat(dpk)], [ops.bsrc(G.sbt_stack[i * r:(i + 1) * r])],
                              [(0, 0, 0, 0, Cc // 64, i * Cc, 0)], lin=True, M=M, N=r, out=dT[:, i * r:(i + 1) * r])
-            with UNetB200._Side(self, (dpk, T, dT, x)):
+            with UNetB200._Side(bw, (dpk, T, dT, x)):
                 for i, L in enumerate(G.layers):
                     self._lora_wgrads(L, M, ops.asrc_mat(dpk[:, i * Cc:(i + 1) * Cc]), ops.asrc_mat(T),
                                       ops.asrc_mat(dT), [(ops.asrc_mat(x), ((0, 0),), (0,))],
@@ -1024,7 +1022,7 @@ class UNetB200:
         ops.gemm(srcs, bs, prog, lin=True, M=M, N=G.cin, out=dx, dep_a_src=None if dT is None else 1)
         return dx
 
-    def conv3_bwd(self, rec, dy, need_dx=True):
+    def conv3_bwd(self, bw, rec, dy, need_dx=True):
         """rec: ConvRec; dy [B,Ho,Wo,N].  Returns dx [B,H,W,cin_total] (or None)."""
         L = self.layers[rec.name]
         B, Ho, Wo, N = dy.shape
@@ -1048,7 +1046,7 @@ class UNetB200:
                            [(sw, sh) for kh, sh in _S2_PLANE[p] for kw, sw in _S2_PLANE[q]],
                            [(kh * 3 + kw) * L.cin for kh, _ in _S2_PLANE[p] for kw, _ in _S2_PLANE[q]])
                           for p in range(2) for q in range(2)]
-            with UNetB200._Side(self, (dy, rec.T, dt, rec.xs)):
+            with UNetB200._Side(bw, (dy, rec.T, dt, rec.xs)):
                 self._lora_wgrads(L, M, ops.asrc_mat(dy_m), ops.asrc_mat(rec.T.view(M, self.r)),
                                   ops.asrc_nhwc(dt), P_list, lin=False, geo=geo)
         if not need_dx:
@@ -1099,7 +1097,7 @@ class UNetB200:
         ops.layernorm_bwd(dy, rec.x, self.layers[rec.name].gamma, rec.stats, add, dx)
         return dx
 
-    def attn_bwd(self, rec, dout):
+    def attn_bwd(self, bw, rec, dout):
         q, k, v, Hh = rec.q, rec.k, rec.v, rec.heads
         D = q.shape[1] // Hh
         Cc = q.shape[1]
@@ -1114,9 +1112,9 @@ class UNetB200:
             assert v.stride(0) == ld and v.storage_offset() == k.storage_offset() + Cc
             dq = self._new(q.shape[0], Cc)
             key = (k.untyped_storage().data_ptr(), ld)
-            if key not in self._dkv_chunks:
-                self._dkv_chunks[key] = self._new(k.shape[0], ld)
-            pk = self._dkv_chunks[key][:, col0:col0 + 2 * Cc]
+            if key not in bw.dkv:
+                bw.dkv[key] = self._new(k.shape[0], ld)
+            pk = bw.dkv[key][:, col0:col0 + 2 * Cc]
             dk, dv = pk[:, :Cc], pk[:, Cc:]
         delta = torch.empty_like(rec.lse)
         ops.attn_bwd(q, k, v, rec.out, dout, rec.lse, delta, dq, dk, dv, rec.B, Hh, rec.Sq, rec.Skv, D, D ** -0.5)
@@ -1125,60 +1123,60 @@ class UNetB200:
     # ------------------------------------------------------------------------------------
     # block backward
     # ------------------------------------------------------------------------------------
-    def resnet_bwd(self, blk, dout, need_dx=True):
+    def resnet_bwd(self, bw, blk, dout, need_dx=True):
         """dout [B,H,W,Cout].  Returns the gradients (NHWC) of the input and of the skip source (None
         without a skip), or (None, None) without need_dx."""
         B, H, W, cout = dout.shape
         M = B * H * W
-        dh2 = self.conv3_bwd(blk.conv2, dout)                          # grad wrt silu(gn2(h1))
+        dh2 = self.conv3_bwd(bw, blk.conv2, dout)                      # grad wrt silu(gn2(h1))
         # grad wrt h1 [M, cout]; its per-image column sums (= d tproj[b, n], the time-embedding
         # branch) are accumulated by the same kernel
         cs32 = self._new(B, cout, dtype=torch.float32)
         dh1, _ = self.gn_bwd(blk.norm2, dh2.view(M, cout), colsum=cs32)
         # the time-embedding branch ends in LoRA weight gradients only: all of it on the side stream
-        with UNetB200._Side(self, (cs32,)):
+        with UNetB200._Side(bw, (cs32,)):
             drow = self._new(B, cout)
             ops.cast_f32_bf16(cs32, drow)
-            self._keep.append(drow)
-            self.linear_bwd(blk.temb, drow, need_dx=False, t_c0=blk.temb.t_c0)
-        dh = self.conv3_bwd(blk.conv1, dh1.view(B, H, W, cout), need_dx=need_dx)
+            bw.keep.append(drow)
+            self.linear_bwd(bw, blk.temb, drow, need_dx=False, t_c0=blk.temb.t_c0)
+        dh = self.conv3_bwd(bw, blk.conv1, dh1.view(B, H, W, cout), need_dx=need_dx)
         dsc = dout.view(M, cout)
         if blk.shortcut is not None:
-            dsc = self.linear_bwd(blk.shortcut, dsc, need_dx=need_dx)
+            dsc = self.linear_bwd(bw, blk.shortcut, dsc, need_dx=need_dx)
         if not need_dx:
             return None, None
         dx1, dx2 = self.gn_bwd(blk.norm1, dh.view(M, -1), add=dsc)
         return dx1.view(B, H, W, -1), None if dx2 is None else dx2.view(B, H, W, -1)
 
-    def transformer_bwd(self, blk, dout):
+    def transformer_bwd(self, bw, blk, dout):
         """dout [B,H,W,C]; returns dx [B,H,W,C]."""
         B, H, W, C = dout.shape
         M = B * H * W
         do = dout.view(M, C)
-        dh = self.linear_bwd(blk.proj_out, do)
+        dh = self.linear_bwd(bw, blk.proj_out, do)
         for b in reversed(blk.blocks):
             dh3 = dh
-            dgg = self.linear_bwd(b.ff_out, dh3)
+            dgg = self.linear_bwd(bw, b.ff_out, dh3)
             du = torch.empty_like(b.geglu.u)
             ops.geglu_bwd(dgg, b.geglu.u, du)
-            dn3 = self.linear_bwd(b.ff_in, du)
+            dn3 = self.linear_bwd(bw, b.ff_in, du)
             dh2 = self.ln_bwd(b.norm3, dn3, add=dh3)
-            da2 = self.linear_bwd(b.attn2_out, dh2)
-            dq2, dkv2 = self.attn_bwd(b.attn2, da2)
-            with UNetB200._Side(self, (dkv2,)):     # feeds weight gradients only: off the dgrad chain
-                self.linear_group_bwd(b.attn2_kv, dkv2, need_dx=False)
-            dn2 = self.linear_bwd(b.attn2_q, dq2)
+            da2 = self.linear_bwd(bw, b.attn2_out, dh2)
+            dq2, dkv2 = self.attn_bwd(bw, b.attn2, da2)
+            with UNetB200._Side(bw, (dkv2,)):     # feeds weight gradients only: off the dgrad chain
+                self.linear_group_bwd(bw, b.attn2_kv, dkv2, need_dx=False)
+            dn2 = self.linear_bwd(bw, b.attn2_q, dq2)
             dh1 = self.ln_bwd(b.norm2, dn2, add=dh2)
-            da1 = self.linear_bwd(b.attn1_out, dh1)
-            _, dqkv = self.attn_bwd(b.attn1, da1)
-            dn1 = self.linear_group_bwd(b.attn1_qkv, dqkv)
+            da1 = self.linear_bwd(bw, b.attn1_out, dh1)
+            _, dqkv = self.attn_bwd(bw, b.attn1, da1)
+            dn1 = self.linear_group_bwd(bw, b.attn1_qkv, dqkv)
             dh = self.ln_bwd(b.norm1, dn1, add=dh1)
-        dg = self.linear_bwd(blk.proj_in, dh)
+        dg = self.linear_bwd(bw, blk.proj_in, dh)
         dx, _ = self.gn_bwd(blk.norm, dg, add=do)
         return dx.view(B, H, W, C)
 
-    def resample_bwd(self, blk, dout):
-        dx = self.conv3_bwd(blk.conv, dout)
+    def resample_bwd(self, bw, blk, dout):
+        dx = self.conv3_bwd(bw, blk.conv, dout)
         if not blk.up:
             return dx
         B, H, W, C = dx.shape
@@ -1192,7 +1190,7 @@ class UNetB200:
         grad_ready(offset): called (on the weight-gradient stream) after each block's backward with
         the flat-buffer offset from which every gradient element is final."""
         tape, head, (B, H, W), rebuild = self.saved
-        self._dkv_chunks = {}
+        bw = _Backward(self.wstream)
         boffs = self.block_grad_offsets() if grad_ready is not None else None
         Lco = self.layers["conv_out"]
         c0 = Lco.cin
@@ -1202,7 +1200,6 @@ class UNetB200:
         d = d.view(B, H, W, c0)
         dskips = []     # gradients of the up path's skip inputs; the last one left (conv_in's output) is unused
         done = None     # the block walked before the current one
-        side = []       # checkpointing: (event, tensors) of the weight-gradient work of the last blocks walked
         for i in reversed(range(len(tape))):
             blk = tape[i]
             if blk.pushes_skip:
@@ -1210,41 +1207,43 @@ class UNetB200:
             # the block walked before has been fully enqueued by now: its gradients are final once the
             # weight-gradient stream drains
             if grad_ready is not None and boffs.get(done) is not None:
-                with UNetB200._Side(self, ()):
+                with UNetB200._Side(bw, ()):
                     grad_ready(boffs[done])
             if isinstance(blk, CheckpointRec):
+                # its forward once more, on the saved student rows with the merged pass's launch plans: every
+                # tensor of the record is bitwise the one the stored tape would hold
                 tape[i] = None              # the rebuilt record holds what the backward still reads
-                blk = self._rebuild(blk, rebuild)
+                blk = self._block(blk.kind, blk.name, blk.xs, rebuild, True, blk.up)[1]
             if isinstance(blk, ResnetRec):
-                d, dskip = self.resnet_bwd(blk, d, need_dx=i > 0)
+                d, dskip = self.resnet_bwd(bw, blk, d, need_dx=i > 0)
                 if blk.takes_skip:
                     dskips.append(dskip)
             elif isinstance(blk, TransformerRec):
-                d = self.transformer_bwd(blk, d)
+                d = self.transformer_bwd(bw, blk, d)
             else:
-                d = self.resample_bwd(blk, d)
+                d = self.resample_bwd(bw, blk, d)
             done = blk.name
             if rebuild is not None:
-                self._release_side(side)
+                self._release_side(bw)
         if grad_ready is not None:
-            with UNetB200._Side(self, ()):
+            with UNetB200._Side(bw, ()):
                 grad_ready(0)
-        self._join_side()
-        side.clear()
+        if bw.wstream is not None:
+            torch.cuda.current_stream().wait_stream(bw.wstream)
         self.saved = None
 
-    def _release_side(self, side):
+    def _release_side(self, bw):
         """Checkpointing: the tensors the weight-gradient stream reads stay referenced (_Side keeps them)
         until that stream is done with them.  Joining the streams after every block would serialise the
         weight gradients with the backward chain, so release them one block late: the current stream
         waits for the side work of the block walked before this one, which has had a whole block's
         backward to finish, and then drops its tensors."""
-        if not self.use_wstream:
+        if bw.wstream is None:
             return
         ev = torch.cuda.Event()
-        ev.record(self.wstream)
-        side.append((ev, self._keep))
-        self._keep = []
-        if len(side) > 1:
-            ev, _ = side.pop(0)
+        ev.record(bw.wstream)
+        bw.side.append((ev, bw.keep))
+        bw.keep = []
+        if len(bw.side) > 1:
+            ev, _ = bw.side.pop(0)
             torch.cuda.current_stream().wait_event(ev)

@@ -132,10 +132,10 @@ def sd15_dry_run():
         mp.setattr(ops, "_call", lambda name, *args: log.append((name, args)))
         block = UNetB200._block
 
-        def marked(self, kind, name, xs, st, ctx, lora, save, up=False):
-            log.append(("block", (kind, name, self._plan_b is not None, "begin")))
-            r = block(self, kind, name, xs, st, ctx, lora, save, up)
-            log.append(("block", (kind, name, self._plan_b is not None, "end")))
+        def marked(self, kind, name, xs, P, save, up=False):
+            log.append(("block", (kind, name, P.plan_b is not None, "begin")))
+            r = block(self, kind, name, xs, P, save, up)
+            log.append(("block", (kind, name, P.plan_b is not None, "end")))
             return r
         mp.setattr(UNetB200, "_block", marked)
         st = PCMTrainStep(config.SD15, weights.synthetic_state_dict(config.SD15, 0), "cpu", batch=B, height=hw,
@@ -145,10 +145,11 @@ def sd15_dry_run():
         bwd = st.unet.backward
 
         def counted(*a, **kw):
-            tape.update(sm.tape_bytes(st.unet.saved))
-            saved["records"] = sm._tensors(st.unet.saved[:2], [])      # block records and the head GN
-            saved["state"] = sm._tensors(st.unet.saved[3], [])         # time embedding, context k / v
-            saved["rows"] = st.unet.saved[2][0]
+            s = st.unet.saved
+            tape.update(sm.tape_bytes(s))
+            saved["records"] = sm._tensors([s.tape, s.head], [])       # block records and the head GN
+            saved["state"] = sm._tensors(s.rebuild, [])                # time embedding, context k / v
+            saved["rows"] = s.shape[0]
             return bwd(*a, **kw)
         st.unet.backward = counted
         log.clear()
@@ -175,7 +176,7 @@ def _segments(log, rebuilding):
     return segs
 
 
-def test_rebuilt_blocks_keep_the_merged_launch_plan(sd15_dry_run):
+def test_rebuilt_blocks_keep_the_merged_pass_launch_plan(sd15_dry_run):
     from pcm_b200 import ops
     log, B = sd15_dry_run["log"], sd15_dry_run["B"]
     merged, rebuilt = _segments(log, False), _segments(log, True)
@@ -202,7 +203,7 @@ def test_rebuilt_blocks_keep_the_merged_launch_plan(sd15_dry_run):
     assert replanned > 0
 
 
-def test_checkpointed_tape_holds_only_student_rows(sd15_dry_run):
+def test_checkpointed_tape_keeps_only_student_rows(sd15_dry_run):
     """SD1.5 bs 8, 64x64: the stored tape keeps about 17 GiB alive (tools/step_memory.py --dry-run); the
     checkpointed one less than 1 GiB, with no storage of a 3B-row activation reachable."""
     tape, saved, B = sd15_dry_run["tape"], sd15_dry_run["saved"], sd15_dry_run["B"]

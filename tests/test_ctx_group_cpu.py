@@ -14,19 +14,18 @@ from gemm_interp import BF16, build_net, interp_gemm as _interp_gemm
 
 @pytest.mark.parametrize("cfg_name", ["TINY", "TINY_XL"])
 @pytest.mark.parametrize("lora_rows", [None, 1])
-def test_context_chunks_equal_per_layer_projections(monkeypatch, cfg_name, lora_rows):
+def test_context_chunks_match_per_layer_projections(monkeypatch, cfg_name, lora_rows):
     from pcm_b200 import config, ops
-    from pcm_b200.unet import UNetB200
+    from pcm_b200.unet import UNetB200, _Pass
     cfg = getattr(config, cfg_name)
     net, sd = build_net(cfg)
     assert net.ctx_group is not None and len(net.ctx_group.chunks) >= 1
     r, s = net.r, net.scale
     B, S = 3, 77
     ctx = torch.randn(B * S, cfg.cross_attention_dim, generator=torch.Generator().manual_seed(5)).to(BF16)
-    net._lb = (lora_rows or B, B)
     Ml = (lora_rows or B) * S
     monkeypatch.setattr(ops, "gemm", _interp_gemm)
-    kv = net.ctx_kv_all(ctx, lora=True)
+    kv = net.ctx_kv_all(_Pass(lora=True, B=B, lb=lora_rows or B, ctx=ctx))
     blocks = [n[:-len(".attn2.to_k")] for n in net._ctx_names if n.endswith(".attn2.to_k")]
     assert sorted(kv) == sorted(blocks)
     seen_windows = set()

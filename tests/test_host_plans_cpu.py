@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from gemm_interp import BF16, build_net, interp_gemm, interp_wgrad as interp_wgrad_, lora_linear_ref
+from pcm_b200.unet import _Backward, _Pass
 
 
 @pytest.fixture(scope="module")
@@ -30,33 +31,33 @@ def _x(rows, cols, seed):
 
 
 @pytest.mark.parametrize("lora_rows", [None, 128])
-def test_linear_with_fused_lora_residual_and_bias(monkeypatch, tiny, lora_rows):
+def test_linear_fuses_lora_residual_and_bias_on_the_pass_rows(monkeypatch, tiny, lora_rows):
     """attn1.to_out.0 (bias, residual) and ff.net.2: T = x A^T as its own launch on the adapter rows, then
     one GEMM with the LoRA block as an extra K entry."""
     from pcm_b200 import ops
     net, sd = tiny
     monkeypatch.setattr(ops, "gemm", interp_gemm)
     M = 384
-    net._lb = (lora_rows or M, M)
+    P = _Pass(lora=True, B=M, lb=lora_rows or M)
     for name in ("down_blocks.0.attentions.0.transformer_blocks.0.attn1.to_out.0",
                  "down_blocks.1.attentions.1.transformer_blocks.0.ff.net.2",
                  "mid_block.attentions.0.proj_in"):
         L = net.layers[name]
         x, res = _x(M, L.cin, 1), _x(M, L.cout, 2)
         tape = []
-        y = net.linear(name, [x], True, residual=res, save=tape)
+        y = net.linear(P, name, [x], residual=res, save=tape)
         ref = lora_linear_ref(sd, name, x, net.scale, lora_rows) + res.float()
         _close(y, ref, name)
         (_, nm, xs, T), = tape
         assert nm == name and T.shape == ((lora_rows or M), net.r) and xs[0].shape[0] == (lora_rows or M)
         # without the adapter: the frozen layer
-        y0 = net.linear(name, [x], False)
+        y0 = net.linear(_Pass(lora=False, B=M, lb=M), name, [x])
         W = sd[name + ".weight"].reshape(L.cout, -1).to(BF16).float()
         _close(y0, x.float() @ W.t() + sd[name + ".bias"].float(), name + " base")
         assert (y.float() - res.float() - y0.float())[: (lora_rows or M)].abs().max() > 1e-2   # the adapter is live
 
 
-def test_linear_over_channel_concatenated_sources(monkeypatch, tiny):
+def test_linear_reads_channel_concatenated_sources(monkeypatch, tiny):
     """conv_shortcut of an up-block resnet: two A sources (hidden state, skip) = torch.cat along channels."""
     from pcm_b200 import ops
     net, sd = tiny
@@ -65,31 +66,29 @@ def test_linear_over_channel_concatenated_sources(monkeypatch, tiny):
     L = net.layers[name]
     c1 = L.cin // 2
     M = 256
-    net._lb = (M, M)
     xa, xb = _x(M, c1, 3), _x(M, L.cin - c1, 4)
-    y = net.linear(name, [xa, xb], True)
+    y = net.linear(_Pass(lora=True, B=M, lb=M), name, [xa, xb])
     _close(y, lora_linear_ref(sd, name, torch.cat([xa, xb], 1), net.scale), name)
 
 
 @pytest.mark.parametrize("lora_rows", [None, 128])
-def test_qkv_group_is_three_lora_linears(monkeypatch, tiny, lora_rows):
+def test_qkv_group_equals_three_lora_linears(monkeypatch, tiny, lora_rows):
     from pcm_b200 import ops
     net, sd = tiny
     monkeypatch.setattr(ops, "gemm", interp_gemm)
     t = "down_blocks.1.attentions.0.transformer_blocks.0"
     G = net.groups[t + ".attn1.to_q"]
     M = 384
-    net._lb = (lora_rows or M, M)
     x = _x(M, G.cin, 7)
     tape = []
-    q, k, v = net.linear_group(t + ".attn1.to_q", x, True, save=tape)
+    q, k, v = net.linear_group(_Pass(lora=True, B=M, lb=lora_rows or M), t + ".attn1.to_q", x, save=tape)
     for suf, got in ((".attn1.to_q", q), (".attn1.to_k", k), (".attn1.to_v", v)):
         _close(got, lora_linear_ref(sd, t + suf, x, net.scale, lora_rows), t + suf)
     assert q.stride(0) == 3 * G.cout and tape[0][3].shape == ((lora_rows or M), 3 * net.r)
 
 
 @pytest.mark.parametrize("lora_rows", [None, 1])
-def test_time_embedding_projections_as_one_group(monkeypatch, tiny, lora_rows):
+def test_time_embedding_projections_run_as_one_group(monkeypatch, tiny, lora_rows):
     """All resnets' time_emb_proj(silu(temb)) from ONE grouped launch: column range i == layer i."""
     from pcm_b200 import ops
     net, sd = tiny
@@ -97,9 +96,8 @@ def test_time_embedding_projections_as_one_group(monkeypatch, tiny, lora_rows):
     G = net.temb_group
     assert G is not None and G.g == len([n for n in net.layers if n.endswith(".time_emb_proj")])
     B = 3
-    net._lb = (lora_rows or B, B)
     st = _x(B, G.cin, 9)
-    out, T = net.temb_all(st, True)
+    out, T = net.temb_all(_Pass(lora=True, B=B, lb=lora_rows or B, st=st))
     assert T.shape == ((lora_rows or B), G.g * net.r)
     for i, name in enumerate(G.names):
         _close(out[:, G.offs[i]:G.offs[i + 1]], lora_linear_ref(sd, name, st, net.scale, lora_rows), name)
@@ -193,7 +191,7 @@ def _rel(got, ref):
     return ((got.double() - ref).norm() / (ref.norm() + 1e-30)).item()
 
 
-def test_linear_backward_plan(monkeypatch, tiny):
+def test_linear_backward_launch_plan(monkeypatch, tiny):
     """linear_bwd: dt = dy (sB), dx = [dy | dt] [W ; A], and the two LoRA weight-gradient launches land in the
     layer's slices of the flat gradient buffer."""
     from pcm_b200 import ops
@@ -203,12 +201,11 @@ def test_linear_backward_plan(monkeypatch, tiny):
     name = "down_blocks.1.attentions.1.transformer_blocks.0.ff.net.2"
     L = net.layers[name]
     M = 256
-    net._lb = (M, M)
     x, dy = _x(M, L.cin, 11), _x(M, L.cout, 12)
     tape = []
-    net.linear(name, [x], True, save=tape)
+    net.linear(_Pass(lora=True, B=M, lb=M), name, [x], save=tape)
     net.lora_grad.zero_()
-    dx = net.linear_bwd(tape[0], dy)
+    dx = net.linear_bwd(_Backward(), tape[0], dy)
     dx_ref, g = _autograd_ref(sd, [name], x, [dy], net.scale, None)
     assert _rel(dx, dx_ref) < 1e-2
     dA, dB = g[name]
@@ -222,7 +219,7 @@ def test_linear_backward_plan(monkeypatch, tiny):
 
 
 @pytest.mark.parametrize("lead,need_dx", [(".attn1.to_q", True), (".attn2.to_k", False)])
-def test_grouped_backward_plan(monkeypatch, tiny, lead, need_dx):
+def test_grouped_backward_launch_plan(monkeypatch, tiny, lead, need_dx):
     """linear_group_bwd over the packed output gradients [dq | dk | dv] (resp. [dk | dv], no input gradient:
     the text context is not trained), with T a column window of a wider stacked down-projection."""
     from pcm_b200 import ops
@@ -232,20 +229,20 @@ def test_grouped_backward_plan(monkeypatch, tiny, lead, need_dx):
     t = "down_blocks.1.attentions.0.transformer_blocks.0"
     G = net.groups[t + lead]
     M = 154 if not need_dx else 256
-    net._lb = (M, M)
     x = _x(M, G.cin, 13)
+    P = _Pass(lora=True, B=M, lb=M, ctx=x)
     dys = [_x(M, G.cout, 20 + i) for i in range(G.g)]
     dpk = torch.cat(dys, 1).contiguous()
     if need_dx:
         tape = []
-        net.linear_group(t + lead, x, True, save=tape)
+        net.linear_group(P, t + lead, x, save=tape)
         rec = tape[0]
     else:
-        kv = net.ctx_kv_all(x, True)            # T = this block's window of the stacked context projection
+        kv = net.ctx_kv_all(P)                  # T = this block's window of the stacked context projection
         rec = ("lgroup", t + lead, x, kv[t][2])
         assert rec[3].stride(0) == net.ctx_group.nl * net.r
     net.lora_grad.zero_()
-    dx = net.linear_group_bwd(rec, dpk, need_dx=need_dx)
+    dx = net.linear_group_bwd(_Backward(), rec, dpk, need_dx=need_dx)
     dx_ref, g = _autograd_ref(sd, G.names, x, dys, net.scale, None)
     if need_dx:
         assert _rel(dx, dx_ref) < 1e-2
@@ -282,42 +279,41 @@ def _img(b, c, h, w, seed):
 
 
 @pytest.mark.parametrize("lora_samples", [None, 1])
-def test_resnet_conv_over_skip_concat_with_row_vector_and_residual(monkeypatch, tiny, lora_samples):
+def test_resnet_conv_reads_skip_concat_row_vector_and_residual(monkeypatch, tiny, lora_samples):
     from pcm_b200 import ops
     net, sd = tiny
     monkeypatch.setattr(ops, "gemm", interp_gemm)
     name = "up_blocks.1.resnets.0.conv1"          # input = cat(hidden, skip)
     L = net.layers[name]
     B, H, W = 3, 8, 8
-    net._lb = (lora_samples or B, B)
     c1 = L.cin // 2
     xa, xb = _img(B, c1, H, W, 31), _img(B, L.cin - c1, H, W, 32)
     rv = _x(B, L.cout, 33)
     res = _img(B, L.cout, H, W, 34)
     tape = []
-    y = net.conv3(name, [_nhwc(xa), _nhwc(xb)], True, rowvec=rv, residual=_nhwc(res), save=tape)
+    y = net.conv3(_Pass(lora=True, B=B, lb=lora_samples or B), name, [_nhwc(xa), _nhwc(xb)], rowvec=rv,
+                  residual=_nhwc(res), save=tape)
     ref, _ = _conv_ref(sd, name, torch.cat([xa, xb], 1).double(), net.scale, 1, lora_samples)
     ref = ref + rv.double()[:, :, None, None] + res.double()
     assert _rel(y.permute(0, 3, 1, 2), ref) < 6e-3
     assert tape[0][3].shape == ((lora_samples or B), H, W, net.r)
 
 
-def test_downsample_conv_reads_the_four_parity_planes(monkeypatch, tiny):
+def test_downsample_conv_reads_four_parity_planes(monkeypatch, tiny):
     from pcm_b200 import ops
     net, sd = tiny
     monkeypatch.setattr(ops, "gemm", interp_gemm)
     name = "down_blocks.0.downsamplers.0.conv"
     L = net.layers[name]
     B, H, W = 2, 8, 8
-    net._lb = (B, B)
     x = _img(B, L.cin, H, W, 35)
-    y = net.conv3(name, [_nhwc(x)], True, stride=2)
+    y = net.conv3(_Pass(lora=True, B=B, lb=B), name, [_nhwc(x)], stride=2)
     ref, _ = _conv_ref(sd, name, x.double(), net.scale, 2)
     assert y.shape == (B, H // 2, W // 2, L.cout) and _rel(y.permute(0, 3, 1, 2), ref) < 6e-3
 
 
 @pytest.mark.parametrize("name,stride", [("down_blocks.1.resnets.0.conv2", 1), ("down_blocks.0.downsamplers.0.conv", 2)])
-def test_conv_backward_plan(monkeypatch, tiny, name, stride):
+def test_conv_backward_launch_plan(monkeypatch, tiny, name, stride):
     """conv3_bwd: dgrad over flipped taps (stride 2: one launch per parity plane of dx, written through a
     strided view), dt = dy (sB), and the tap-wise LoRA weight gradients - against float64 autograd."""
     from pcm_b200 import ops
@@ -326,13 +322,12 @@ def test_conv_backward_plan(monkeypatch, tiny, name, stride):
     monkeypatch.setattr(ops, "wgrad", interp_wgrad_)
     L = net.layers[name]
     B, H, W = 2, 8, 8
-    net._lb = (B, B)
     x = _img(B, L.cin, H, W, 41)
     dy = _img(B, L.cout, H // stride, W // stride, 42)
     tape = []
-    net.conv3(name, [_nhwc(x)], True, stride=stride, save=tape)
+    net.conv3(_Pass(lora=True, B=B, lb=B), name, [_nhwc(x)], stride=stride, save=tape)
     net.lora_grad.zero_()
-    dx = net.conv3_bwd(tape[0], _nhwc(dy))
+    dx = net.conv3_bwd(_Backward(), tape[0], _nhwc(dy))
     x64 = x.double().requires_grad_(True)
     F = torch.nn.functional
     Wt = sd[name + ".weight"].to(BF16).double()

@@ -69,7 +69,7 @@ def test_forward_and_backward_match_the_oracle(monkeypatch, cfg_name):
     assert (num / den) ** 0.5 <= 5e-2, (num / den) ** 0.5
 
 
-def test_merged_pass_is_student_plus_frozen_teacher(monkeypatch):
+def test_merged_pass_equals_student_plus_frozen_teacher(monkeypatch):
     """lora_batch = b < B: the leading b samples see the adapter, the others the frozen network, in ONE
     pass; the tape then belongs to the student samples and backward() gives the student's gradients."""
     B, hw = 3, 8
@@ -80,7 +80,7 @@ def test_merged_pass_is_student_plus_frozen_teacher(monkeypatch):
     ctx2 = ctx.reshape(B * S, -1)
     ts = torch.tensor([999, 19, 499])
     merged = net.forward(x, ts, ctx2, lora=True, save=True, lora_batch=1)
-    kv = net.last_ctx_kv
+    kv = net.saved_ctx_kv()
     G = torch.randn(1, hw, hw, 4, generator=torch.Generator().manual_seed(8)) / (4 * hw * hw)
     net.lora_grad.zero_()
     net.backward(G)

@@ -66,7 +66,7 @@ def block_inputs(saved):
     """The student rows of every block input on a tape (stored or checkpointed), one entry per tensor."""
     from pcm_b200.unet import CheckpointRec, ResampleRec, ResnetRec, TransformerRec
     seen, out = set(), []
-    for blk in saved[0]:
+    for blk in saved.tape:
         if isinstance(blk, CheckpointRec):
             xs, div = blk.xs, 1
         elif isinstance(blk, ResnetRec):
