@@ -731,6 +731,8 @@ extern "C" int pcm_groupnorm_bwd(const void* dy_, const void* x1_, const void* x
   (void)eps;  // folded into stats (mean, rstd) by the forward
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const int C = C1 + C2;
+  // the same channel split as the forward: each thread's 16-byte vectors must lie in x1 or x2 entirely
+  if (C % G != 0 || C1 % 8 != 0 || C2 % 8 != 0) return set_error("groupnorm: bad channel split");
   if (B > kGnMaxB) return set_error("groupnorm: batch too large for the counter workspace");
   const bf16* dy = reinterpret_cast<const bf16*>(dy_);
   const bf16* x1 = reinterpret_cast<const bf16*>(x1_);
