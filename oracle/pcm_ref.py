@@ -66,12 +66,17 @@ class DDIMSolverRef:
             np.asarray([alpha_cumprods[0]] + alpha_cumprods[ts[:-1]].tolist()))
         self.ddim_timesteps = torch.from_numpy(ts).long()
 
+    def to(self, device):
+        for k in ("ddim_alpha_cumprods", "ddim_timesteps_prev", "ddim_alpha_cumprods_prev", "ddim_timesteps"):
+            setattr(self, k, getattr(self, k).to(device))
+        return self
+
     def ddim_step(self, pred_x0, pred_noise, timestep_index):  # T15:313-319
         a = extract_into_tensor(self.ddim_alpha_cumprods_prev, timestep_index, pred_x0.shape)
         return a.sqrt() * pred_x0 + (1.0 - a).sqrt() * pred_noise
 
     def ddim_style_multiphase_pred(self, pred_x0, pred_noise, timestep_index, multiphase):  # T15:321-341
-        inf = torch.from_numpy(inference_indices(len(self.ddim_timesteps), multiphase)).long()
+        inf = torch.from_numpy(inference_indices(len(self.ddim_timesteps), multiphase)).long().to(timestep_index.device)
         # largest phase-start index <= timestep_index  (expand / >= / flip / argmax in the reference)
         pos = (timestep_index[:, None] >= inf[None, :]).long().sum(1) - 1
         p = inf[pos]
@@ -101,32 +106,42 @@ def noise_travel(alphas_cumprod, x, noise, t_cur, t_tgt):  # S15:526-554
 
 def pcm_step_ref(cfg, params, batch, *, multiphase, num_ddim=50, loss_type="huber", huber_c=1e-3,
                  prediction_type="epsilon", apply_cfg_solver=True, emulate_bf16=False,
-                 need_grad=True, round_eps_bf16=None, teacher_substeps=1):
+                 need_grad=True, round_eps_bf16=None, teacher_substeps=1, round_inputs=None,
+                 round_grads=False):
     """One iteration of the reference loop, T15:1139-1293, on explicit inputs.
 
     batch: latents [B,4,H,W], noise, index [B] int64, w [B], prompt_embeds [B,77,D],
-           uncond_prompt_embeds [B,77,D]  (all fp32 CPU tensors)
+           uncond_prompt_embeds [B,77,D]  (fp32 tensors, or tensors of the parameters' dtype; the step
+           runs on the latents' device)
+    round_inputs (default: emulate_bf16): keep latents, noise and w in bf16 and add the noise in bf16,
+    like the reference under mixed precision; True with emulate_bf16=False gives an unrounded network
+    on the inputs the bf16 step sees.  round_grads: UNetRef's bf16 rounding of the backward.
     Returns dict(loss, grads{name: tensor}, model_pred, target, x_prev, eps_student, ...).
     The target network is the SAME LoRA student under no_grad (T15:1261-1268; update_ema is never
     called in the reference)."""
+    dev = batch["latents"].device
     ac = sd15_alphas_cumprod()
+    solver = DDIMSolverRef(ac.numpy(), 1000, num_ddim).to(dev)                # T15:811-815
+    ac = ac.to(dev)
     alpha_schedule, sigma_schedule = torch.sqrt(ac), torch.sqrt(1 - ac)      # T15:808-809
-    solver = DDIMSolverRef(ac.numpy(), 1000, num_ddim)                        # T15:811-815
     if round_eps_bf16 is None:
         round_eps_bf16 = emulate_bf16
+    if round_inputs is None:
+        round_inputs = emulate_bf16
     P = dict(params)
     lk = lora_keys(P)
     if need_grad:
         for k in lk:
             P[k] = P[k].detach().clone().requires_grad_(True)
-    student = UNetRef(cfg, P, use_lora=True, emulate_bf16=emulate_bf16)
+    student = UNetRef(cfg, P, use_lora=True, emulate_bf16=emulate_bf16, round_grads=round_grads)
     teacher = UNetRef(cfg, P, use_lora=False, emulate_bf16=emulate_bf16)
+    fdt = next(iter(P.values())).dtype
 
     def rq(x):  # dtype of tensors the reference keeps in weight_dtype (bf16 under mixed precision)
-        return x.to(torch.bfloat16).float() if emulate_bf16 else x
+        return x.to(torch.bfloat16).to(fdt) if round_inputs else x
 
     latents, noise = rq(batch["latents"]), rq(batch["noise"])                 # T15:1136, 1139
-    index, w = batch["index"], batch["w"]
+    index, w = batch["index"].to(dev), batch["w"].to(dev)
     prompt, uncond = batch["prompt_embeds"], batch["uncond_prompt_embeds"]
     # SDXL (train_pcm_lora_sdxl_adv.py:1094-1133, 1215-1221): added_cond_kwargs; the unconditional
     # teacher pass uses ZERO pooled text embeddings and the same time ids
@@ -137,11 +152,11 @@ def pcm_step_ref(cfg, params, batch, *, multiphase, num_ddim=50, loss_type="hube
     topk = 1000 // num_ddim                                                   # T15:1143-1146
     start_t = solver.ddim_timesteps[index]                                    # T15:1151
     t = torch.clamp(start_t - topk, min=0)                                    # T15:1152-1155
-    inf = torch.from_numpy(inference_indices(num_ddim, multiphase)).long()    # T15:1157-1163
+    inf = torch.from_numpy(inference_indices(num_ddim, multiphase)).long().to(dev)  # T15:1157-1163
     c_skip_s, c_out_s = [append_dims(x, 4) for x in scalings_for_boundary_conditions_online(index, inf)]
     c_skip, c_out = [append_dims(x, 4) for x in scalings_for_boundary_conditions_target(index, inf)]
-    if emulate_bf16:   # latents are weight_dtype (bf16) tensors in the reference: run its exact op sequence
-        noisy = add_noise(ac, latents.bfloat16(), noise.bfloat16(), start_t).float()
+    if round_inputs:   # latents are weight_dtype (bf16) tensors in the reference: run its exact op sequence
+        noisy = add_noise(ac, latents.bfloat16(), noise.bfloat16(), start_t).to(fdt)
     else:
         noisy = add_noise(ac, latents, noise, start_t)                        # T15:1178
     w4 = rq(w.reshape(-1, 1, 1, 1))                                           # T15:1183-1185
@@ -175,7 +190,7 @@ def pcm_step_ref(cfg, params, batch, *, multiphase, num_ddim=50, loss_type="hube
                 if j == k - 1:
                     x_prev = x_next
                     break
-                x_cur, t_cur = x_next.float(), t_next.clamp(min=0)
+                x_cur, t_cur = x_next.to(fdt), t_next.clamp(min=0)
                 e_c = teacher(x_cur, t_cur, prompt, addc)
                 e_u = teacher(x_cur, t_cur, uncond, addu) if apply_cfg_solver else e_c
                 p_c = predicted_origin(e_c, t_cur, x_cur, prediction_type, alpha_schedule, sigma_schedule)
@@ -183,15 +198,15 @@ def pcm_step_ref(cfg, params, batch, *, multiphase, num_ddim=50, loss_type="hube
                 pred_x0 = p_c + w4 * (p_c - p_u)
                 pred_noise = e_c + w4 * (e_c - e_u)
 
-        eps_t = student(x_prev.float(), t, prompt, addc)                      # T15:1263-1268
+        eps_t = student(x_prev.to(fdt), t, prompt, addc)                      # T15:1263-1268
         x0_t = predicted_origin(eps_t, t, x_prev, prediction_type, alpha_schedule, sigma_schedule)
         target, end_t2 = solver.ddim_style_multiphase_pred(x0_t, eps_t, index, multiphase)
         target = c_skip * x_prev + c_out * target                             # T15:1280
 
     if loss_type == "l2":                                                     # T15:1283-1293
-        loss = torch.nn.functional.mse_loss(model_pred.float(), target.float(), reduction="mean")
+        loss = torch.nn.functional.mse_loss(model_pred.to(fdt), target.to(fdt), reduction="mean")
     else:
-        loss = torch.mean(torch.sqrt((model_pred.float() - target.float()) ** 2 + huber_c ** 2) - huber_c)
+        loss = torch.mean(torch.sqrt((model_pred.to(fdt) - target.to(fdt)) ** 2 + huber_c ** 2) - huber_c)
     out = dict(loss=loss.detach(), model_pred=model_pred.detach(), target=target.detach(),
                x_prev=x_prev.detach(), eps_student=eps.detach(), eps_cond=eps_c, eps_uncond=eps_u,
                eps_target=eps_t, noisy=noisy, start_timesteps=start_t, timesteps=t, end_timesteps=end_t)

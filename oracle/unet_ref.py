@@ -18,6 +18,10 @@ prefix and ``.default`` infix).
 
 ``emulate_bf16=True`` rounds weights and every tensor the CUDA path materialises in HBM to bf16
 (straight-through in autograd); this mirrors the reference running under bf16 autocast.
+``round_grads=True`` (with emulate_bf16) also rounds, in the backward, the gradient of every tensor whose
+gradient the CUDA backward stores in bf16 (see UNetRef).
+
+The network runs on the device and in the dtype of its parameters (float64 on CUDA included).
 """
 import math
 from dataclasses import dataclass
@@ -207,19 +211,43 @@ def lora_keys(P):
 # ---------------------------------------------------------------------------------------------
 # forward
 # ---------------------------------------------------------------------------------------------
-def _q(x, on):
-    """bf16 rounding with a straight-through gradient."""
+def _round_grad(g):
+    return g.to(torch.bfloat16).to(g.dtype)
+
+
+def _q(x, on, grad=False):
+    """bf16 rounding with a straight-through gradient; grad=True also rounds the gradient to bf16 (a hook:
+    the forward is the same tensor either way)."""
     if not on:
         return x
-    return x + (x.to(torch.bfloat16).to(x.dtype) - x).detach()
+    y = x + (x.to(torch.bfloat16).to(x.dtype) - x).detach()
+    if grad and y.requires_grad:
+        y.register_hook(_round_grad)
+    return y
+
+
+def _qg(x, on):
+    """x itself, its gradient rounded to bf16 (a hook on x: only for a tensor that has this one use)."""
+    if on and x.requires_grad:
+        x.register_hook(_round_grad)
+    return x
 
 
 class UNetRef:
-    """Functional UNet over a flat parameter dict.  use_lora=False gives the frozen teacher."""
+    """Functional UNet over a flat parameter dict.  use_lora=False gives the frozen teacher.
+
+    round_grads (with emulate_bf16) rounds the gradients the CUDA backward (pcm_b200/unet.py) stores in
+    bf16: those of every GEMM output but eps (conv_out's input gradient is computed from the fp32 d_eps),
+    of every LoRA down-projection T, GroupNorm / LayerNorm output, attention output and GEGLU output, of
+    a skip concatenation (add_bf16 then sums two bf16 gradients) and of an upsampler's nearest-neighbour
+    output (upsample2x_bwd sums four bf16 gradients).  A time-embedding row vector takes its gradient
+    before the rounding: the GroupNorm backward sums it over the pixels in fp32.  The softmax probabilities are
+    left alone: the flash backward never stores dP, it rounds dS = P (dP - delta) in registers."""
 
     def __init__(self, cfg: UNetConfig, params: Dict[str, torch.Tensor], use_lora: bool = True,
-                 emulate_bf16: bool = False):
+                 emulate_bf16: bool = False, round_grads: bool = False):
         self.cfg, self.P, self.use_lora, self.emu = cfg, params, use_lora, emulate_bf16
+        self.rg = emulate_bf16 and round_grads
         self.scale = cfg.lora_alpha / cfg.lora_rank
         self.taps = {}  # optional activation taps for layer-wise parity tests
 
@@ -227,38 +255,44 @@ class UNetRef:
     def w(self, name):
         return _q(self.P[name], self.emu)
 
-    def conv(self, name, x, stride=1, extra=None):
-        """Conv2d (+ peft LoRA branch) (+ fused additive terms), rounded once like the GEMM epilogue."""
+    def conv(self, name, x, stride=1, extra=None, rowvec=None):
+        """Conv2d (+ peft LoRA branch) (+ fused additive terms), rounded once like the GEMM epilogue.
+        rowvec: a per-sample [B, C, 1, 1] term (the time embedding); the GroupNorm backward sums its
+        gradient in fp32 before it rounds the convolution's output gradient."""
         W = self.w(name + ".weight")
         k = W.shape[-1]
         y = F.conv2d(x, W, self.P.get(name + ".bias"), stride=stride, padding=k // 2)
         if self.use_lora and (name + ".lora_A.weight") in self.P:
             t = F.conv2d(x, self.w(name + ".lora_A.weight"), None, stride=stride, padding=k // 2)
-            t = _q(t, self.emu)
+            t = _q(t, self.emu, self.rg)
             y = y + F.conv2d(t, self.w(name + ".lora_B.weight") * self.scale)
         if extra is not None:
             y = y + extra
-        return _q(y, self.emu)
+        if rowvec is not None:
+            y = _qg(y, self.rg) + rowvec
+            return _q(y, self.emu)
+        return _q(y, self.emu, self.rg and name != "conv_out")
 
     def linear(self, name, x, extra=None, act=None):
         y = F.linear(x, self.w(name + ".weight"), self.P.get(name + ".bias"))
         if self.use_lora and (name + ".lora_A.weight") in self.P:
-            t = _q(F.linear(x, self.w(name + ".lora_A.weight")), self.emu)
+            t = _q(F.linear(x, self.w(name + ".lora_A.weight")), self.emu, self.rg)
             y = y + F.linear(t, self.w(name + ".lora_B.weight") * self.scale)
         if extra is not None:
             y = y + extra
         if act == "silu":
             y = F.silu(y)
-        return _q(y, self.emu)
+        return _q(y, self.emu, self.rg)
 
     def gn(self, name, x, eps, silu):
         y = F.group_norm(x, self.cfg.norm_num_groups, self.P[name + ".weight"], self.P[name + ".bias"], eps)
         if silu:
             y = F.silu(y)
-        return _q(y, self.emu)
+        return _q(y, self.emu, self.rg)
 
     def ln(self, name, x):
-        return _q(F.layer_norm(x, (x.shape[-1],), self.P[name + ".weight"], self.P[name + ".bias"], 1e-5), self.emu)
+        return _q(F.layer_norm(x, (x.shape[-1],), self.P[name + ".weight"], self.P[name + ".bias"], 1e-5), self.emu,
+                  self.rg)
 
     def attention(self, q, k, v, H=None):
         B, S, Cc = q.shape
@@ -275,14 +309,14 @@ class UNetRef:
             p = _q(p, self.emu)  # the flash kernels feed bf16 probabilities to the PV product
             outs.append(p @ v)
         o = (outs[0] if len(outs) == 1 else torch.cat(outs, dim=2)).transpose(1, 2).reshape(B, S, Cc)
-        return _q(o, self.emu)
+        return _q(o, self.emu, self.rg)
 
     # -- blocks -----------------------------------------------------------------------------
     def resnet(self, p, x, st):
         cin, cout = x.shape[1], self.P[p + ".conv1.weight"].shape[0]
         h = self.gn(p + ".norm1", x, 1e-5, True)
         tproj = self.linear(p + ".time_emb_proj", st)                       # [B, cout]
-        h = self.conv(p + ".conv1", h, extra=tproj[:, :, None, None])
+        h = self.conv(p + ".conv1", h, rowvec=tproj[:, :, None, None])
         h = self.gn(p + ".norm2", h, 1e-5, True)
         sc = self.conv(p + ".conv_shortcut", x) if cin != cout else x
         return self.conv(p + ".conv2", h, extra=sc)
@@ -314,7 +348,7 @@ class UNetRef:
             n = self.ln(t + ".norm3", h)
             u = self.linear(t + ".ff.net.0.proj", n)
             a_, g_ = u.chunk(2, dim=-1)
-            gg = _q(a_ * F.gelu(g_), self.emu)                               # GEGLU, exact-erf GELU
+            gg = _q(a_ * F.gelu(g_), self.emu, self.rg)                      # GEGLU, exact-erf GELU
             h = self.linear(t + ".ff.net.2", gg, extra=h)
         if self.cfg.use_linear_projection:
             h = self.linear(p + ".proj_out", h, extra=r.permute(0, 2, 3, 1).reshape(B, Hh * Ww, Cc))
@@ -324,8 +358,9 @@ class UNetRef:
 
     def _sinusoid(self, values, dim):
         half = dim // 2
-        f = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=torch.float32) / half)
-        e = values[:, None].float() * f[None]
+        dt = self.P["conv_in.weight"].dtype
+        f = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=dt, device=values.device) / half)
+        e = values[:, None].to(dt) * f[None]
         return torch.cat([torch.cos(e), torch.sin(e)], dim=-1)               # flip_sin_to_cos, shift 0
 
     def time_embed(self, timesteps, added_cond_kwargs=None):
@@ -340,7 +375,7 @@ class UNetRef:
         text_embeds, time_ids = added_cond_kwargs["text_embeds"], added_cond_kwargs["time_ids"]
         B = time_ids.shape[0]
         tid = self._sinusoid(time_ids.flatten(), self.cfg.addition_time_embed_dim).reshape(B, -1)
-        add = _q(torch.cat([text_embeds.float(), tid], dim=-1), self.emu)
+        add = _q(torch.cat([text_embeds.to(tid.dtype), tid], dim=-1), self.emu)
         a = self.linear("add_embedding.linear_1", add, act="silu")
         return self.linear("add_embedding.linear_2", a, extra=temb, act="silu")
 
@@ -370,12 +405,12 @@ class UNetRef:
         self.taps["mid"] = x
         for i in range(nb):
             for j in range(cfg.layers_per_block + 1):
-                x = torch.cat([x, skips.pop()], dim=1)
+                x = _qg(torch.cat([x, skips.pop()], dim=1), self.rg)
                 x = self.resnet(f"up_blocks.{i}.resnets.{j}", x, st)
                 if cfg.up_attn[i]:
                     x = self.transformer(f"up_blocks.{i}.attentions.{j}", x, ctx, nb - 1 - i)
             if i < nb - 1:
-                x = F.interpolate(x, scale_factor=2.0, mode="nearest")
+                x = _qg(F.interpolate(x, scale_factor=2.0, mode="nearest"), self.rg)
                 x = self.conv(f"up_blocks.{i}.upsamplers.0.conv", x)
         x = self.gn("conv_norm_out", x, 1e-5, True)
         return self.conv("conv_out", x)
