@@ -131,10 +131,15 @@ int pcm_num_sms(void);
  * pointer aligned to its element.
  * pcm_wgrad: M < 1, a null out, os_row or os_col of zero; out 4-byte aligned, and with os_col == 1 (ranks
  * added in pairs) 8-byte aligned with even os_row and tap_off.
- * pcm_gemm_check / pcm_wgrad_check run exactly those checks and launch nothing. */
+ * pcm_gemm_check / pcm_wgrad_check run exactly those checks and launch nothing.
+ * pcm_gemm_plan_rows: the output rows per CTA tile pcm_gemm runs the descriptor with, 128 or 256 (256 for
+ * block_n 128 / 160 launches that run unsplit, whose entries without an N or M range hold at least 32 K
+ * blocks, whose M-ranged entries end on 256-row boundaries and whose 256-row tiles need at most half the
+ * waves of 128-row ones); launches nothing. */
 int pcm_gemm(const pcm_gemm_desc* d, void* stream);
 int pcm_wgrad(const pcm_wgrad_desc* d, void* stream);
 int pcm_gemm_check(const pcm_gemm_desc* d);
+int pcm_gemm_plan_rows(const pcm_gemm_desc* d);
 int pcm_wgrad_check(const pcm_wgrad_desc* d);
 
 /* ---- GroupNorm(+SiLU) / LayerNorm (NHWC bf16; fp32 statistics) ----------------------------

@@ -86,6 +86,7 @@ EXPORTS = [
     "pcm_wgrad",
     "pcm_gemm_check",
     "pcm_wgrad_check",
+    "pcm_gemm_plan_rows",
     "pcm_groupnorm_ws_bytes",
     "pcm_groupnorm_fwd",
     "pcm_groupnorm_fwd_part",
@@ -126,6 +127,7 @@ ARGTYPES = {
     "pcm_wgrad": [P, P],
     "pcm_gemm_check": [P],
     "pcm_wgrad_check": [P],
+    "pcm_gemm_plan_rows": [P],
     "pcm_groupnorm_ws_bytes": [I, I, I, I],
     "pcm_groupnorm_fwd": [P, P, I, I, I, I, I, P, P, F, I, P, P, P, L64, P],
     "pcm_groupnorm_fwd_part": [P, P, I, I, I, I, I, I, P, P, F, I, P, P, P, L64, P],

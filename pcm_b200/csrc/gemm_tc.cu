@@ -13,10 +13,12 @@
 // Replaces the cuDNN / cuBLAS calls that diffusers' UNet2DConditionModel + peft LoRA issue for
 // train_pcm_lora_sd15.py:1192-1198, 1219-1223, 1238-1244, 1263-1268 (forwards) and :1296
 // (backward).  Warpgroup roles: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 =
-// consumers, each owning 64 rows of the 128 x BN output tile: wgmma into registers, then the
-// epilogue from those registers (gemm_epilogue.cuh) while the producer already fills the stages of
-// the next tile.  BN (the N tile, a multiple of 32 up to 256) is a template parameter: it is the N
-// of the wgmma instruction.
+// consumers, each owning 64 * MS rows of the (128 * MS) x BN output tile: wgmma into registers, then
+// the epilogue from those registers (gemm_epilogue.cuh) while the producer already fills the stages
+// of the next tile.  BN (the N tile, a multiple of 32 up to 256) is a template parameter: it is the N
+// of the wgmma instruction.  MS (1 or 2) is the number of 128-row A slabs per stage: with MS = 2 a
+// consumer runs two m64 accumulators against the same weight tile, so each B tile brought into
+// shared memory feeds 256 rows instead of 128 (gemm_plan_rows picks it).
 // K-program entries may be restricted to an output-column range (grouped Linear layers sharing
 // their input) or to the leading M tiles (an A source with fewer rows than the output: the LoRA
 // T of the student samples in the merged student + teacher pass).  Weights may be K-blocked
@@ -58,7 +60,7 @@ __device__ __forceinline__ int chunk_ksteps(int kend, int c) {
 // NARROW: some K chunk of the program is narrower than 64 (a LoRA rank r % 64 != 0); the producer
 // publishes each stage's k16 step count and the consumers issue only those.  Launches without a
 // narrow chunk run the plain 4-step mainloop.
-template <int BN, bool NARROW>
+template <int BN, int MS, bool NARROW>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -70,7 +72,8 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
 
   const int wg = threadIdx.x >> 7;
   const int S = p.num_stages;
-  constexpr uint32_t stage_bytes = kATileBytes + BN * 128;
+  constexpr int kRows = 128 * MS;   // output rows of a tile
+  constexpr uint32_t stage_bytes = MS * kATileBytes + BN * 128;
   const int num_items = p.tiles_m * p.tiles_n * p.ksplit;
   const int kb_per = (p.num_kblocks + p.ksplit - 1) / p.ksplit;
 
@@ -93,7 +96,7 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
 
   if (wg == 0) {
     // ===================== TMA producer =====================
-    regs_dealloc<40>();
+    regs_dealloc<MS == 2 ? 24 : 40>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -104,11 +107,14 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
         int tm = tile / p.tiles_n;
         const int tn = tile - tm * p.tiles_n;
         if (p.dep_a_map >= 0) tm = p.tiles_m - 1 - tm;  // adapter-free rows first (see dep_a_src1)
-        const int m0 = tm * 128, n0 = tn * BN;
-        int b0 = 0, h0 = 0;
+        const int m0 = tm * kRows, n0 = tn * BN;
+        int b0[MS] = {}, h0[MS] = {};   // conv mode: TMA coordinates of each 128-row slab
         if (!p.lin) {
-          b0 = m0 / p.geoHW;
-          h0 = (m0 - b0 * p.geoHW) / p.geoW;
+#pragma unroll
+          for (int s = 0; s < MS; ++s) {
+            b0[s] = (m0 + 128 * s) / p.geoHW;
+            h0[s] = (m0 + 128 * s - b0[s] * p.geoHW) / p.geoW;
+          }
         }
         int kidx = 0;
         for (int e = 0; e < p.num_prog; ++e) {
@@ -130,12 +136,17 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
             if constexpr (NARROW) stage_ksteps[stage] = chunk_ksteps(en.kend, c);
             mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
             uint8_t* sa = smem + stage * stage_bytes;
-            uint8_t* sb = sa + kATileBytes;
-            if (p.lin)
-              tma_load_4d(sa, &p.a_maps[en.a_map], &full_bar[stage], en.a_c0 + c * 64, m0, 0, 0);
-            else
-              tma_load_4d(sa, &p.a_maps[en.a_map], &full_bar[stage], en.a_c0 + c * 64, en.dw,
-                          h0 + en.dh, b0);
+            uint8_t* sb = sa + MS * kATileBytes;
+            // a slab past M (past the last image) is zero-filled by TMA; the epilogue skips its rows
+#pragma unroll
+            for (int s = 0; s < MS; ++s) {
+              if (p.lin)
+                tma_load_4d(sa + s * kATileBytes, &p.a_maps[en.a_map], &full_bar[stage], en.a_c0 + c * 64,
+                            m0 + 128 * s, 0, 0);
+              else
+                tma_load_4d(sa + s * kATileBytes, &p.a_maps[en.a_map], &full_bar[stage], en.a_c0 + c * 64,
+                            en.dw, h0[s] + en.dh, b0[s]);
+            }
             if ((p.b_blocked >> en.b_map) & 1)   // K-blocked weights: (64, N, K/64) view, contiguous tile
               tma_load_3d(sb, &p.b_maps[en.b_map], &full_bar[stage], 0, n0, (en.b_k0 >> 6) + c);
             else
@@ -150,11 +161,11 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
     }
   } else {
     // ===================== consumers: wgmma mainloop + epilogue =====================
-    regs_alloc<232>();   // 128 x 40 + 256 x 232 <= 64 K registers
-    const int cw = wg - 1;                 // rows cw * 64 .. cw * 64 + 63 of the tile
+    regs_alloc<MS == 2 ? 240 : 232>();   // 128 x 40 + 256 x 232 (128 x 24 + 256 x 240) <= 64 K registers
+    const int cw = wg - 1;                 // rows cw * 64 * MS .. of the tile: MS slabs of 64 rows
     const int et = threadIdx.x & 127;
     float* sbuf = reinterpret_cast<float*>(smem + S * stage_bytes) + cw * (64 * 32);
-    float acc[BN / 2];
+    float acc[MS][BN / 2];
     int stage = 0;
     uint32_t phase = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
@@ -163,33 +174,41 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
       const int tn = tile - tm * p.tiles_n;
       if (p.dep_a_map >= 0) tm = p.tiles_m - 1 - tm;
       const int n0 = tn * BN;
-      const int nkb = p.filtered ? tile_kblocks(p, tm * 128, n0)   // N- or M-ranged entries (ksplit == 1)
+      const int nkb = p.filtered ? tile_kblocks(p, tm * kRows, n0)   // N- or M-ranged entries (ksplit == 1)
                                  : min(p.num_kblocks, (ks + 1) * kb_per) - ks * kb_per;
       if (nkb <= 0) {
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int s = 0; s < MS; ++s)
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[s][i] = 0.f;
       }
       int prev_stage = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        const uint32_t a_addr = smem_u32(smem + stage * stage_bytes) + cw * (64 * 128);
-        const uint32_t b_addr = smem_u32(smem + stage * stage_bytes) + kATileBytes;
+        // slab s of this warpgroup: A rows (MS cw + s) * 64 .. of the stage, 8 KB each
+        const uint32_t a_addr = smem_u32(smem + stage * stage_bytes) + cw * MS * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + stage * stage_bytes) + MS * kATileBytes;
         wgmma_fence();
         if constexpr (NARROW) {
           const int nk = stage_ksteps[stage];   // warpgroup-uniform
 #pragma unroll
           for (int k = 0; k < 4; ++k)
             if (k < nk)
-              Wgmma<BN, 0, 0>::mma(acc, wgmma_desc_sw128(a_addr + k * 32, 16, 1024),
-                                   wgmma_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
+#pragma unroll
+              for (int s = 0; s < MS; ++s)
+                Wgmma<BN, 0, 0>::mma(acc[s], wgmma_desc_sw128(a_addr + s * (64 * 128) + k * 32, 16, 1024),
+                                     wgmma_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
         } else {
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-            Wgmma<BN, 0, 0>::mma(acc, wgmma_desc_sw128(a_addr + k * 32, 16, 1024),
-                                 wgmma_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
+#pragma unroll
+            for (int s = 0; s < MS; ++s)
+              Wgmma<BN, 0, 0>::mma(acc[s], wgmma_desc_sw128(a_addr + s * (64 * 128) + k * 32, 16, 1024),
+                                   wgmma_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0 ? 1u : 0u);
         }
         wgmma_commit();
-        wgmma_fence_acc(acc);
+#pragma unroll
+        for (int s = 0; s < MS; ++s) wgmma_fence_acc(acc[s]);
         // the previous K block's wgmma are complete: its stage may be refilled
         wgmma_wait<1>();
         if (prev_stage >= 0 && et == 0) mbar_arrive(&empty_bar[prev_stage]);
@@ -200,11 +219,14 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
         }
       }
       wgmma_wait<0>();
-      wgmma_fence_acc(acc);
+#pragma unroll
+      for (int s = 0; s < MS; ++s) wgmma_fence_acc(acc[s]);
       if (prev_stage >= 0 && et == 0) mbar_arrive(&empty_bar[prev_stage]);
       // split-K: this item's partial sums go to slice ks of the workspace
       float* ws = p.ws ? p.ws + static_cast<long long>(ks) * p.M * p.N : nullptr;
-      gemm_epilogue_tile<BN>(p, tm * 128 + cw * 64, n0, acc, sbuf, et, 1 + cw, ws);
+#pragma unroll
+      for (int s = 0; s < MS; ++s)
+        gemm_epilogue_tile<BN>(p, tm * kRows + (cw * MS + s) * 64, n0, acc[s], sbuf, et, 1 + cw, ws);
     }
   }
 }
@@ -452,19 +474,21 @@ static int encode_asrc(CUtensorMap* map, const pcm_asrc& a, int lin, int geoW, i
   return encode_tmap(map, a.ptr, 4, dims, strides, box, estr);
 }
 
-// the wgmma N of the kernel is the N tile of the launch
+// the wgmma N of the kernel is the N tile of the launch; 256-row tiles exist for BN = 128 and 160 only
+// (gemm_plan_rows never picks them elsewhere)
 typedef void (*GemmKernel)(const GemmParams);
 template <bool NARROW>
-static GemmKernel gemm_kernel_for(int block_n) {
+static GemmKernel gemm_kernel_for(int block_n, int rows) {
+  if (rows == 256) return block_n == 128 ? pcm_gemm_kernel<128, 2, NARROW> : pcm_gemm_kernel<160, 2, NARROW>;
   switch (block_n) {
-    case 32: return pcm_gemm_kernel<32, NARROW>;
-    case 64: return pcm_gemm_kernel<64, NARROW>;
-    case 96: return pcm_gemm_kernel<96, NARROW>;
-    case 128: return pcm_gemm_kernel<128, NARROW>;
-    case 160: return pcm_gemm_kernel<160, NARROW>;
-    case 192: return pcm_gemm_kernel<192, NARROW>;
-    case 224: return pcm_gemm_kernel<224, NARROW>;
-    default: return pcm_gemm_kernel<256, NARROW>;
+    case 32: return pcm_gemm_kernel<32, 1, NARROW>;
+    case 64: return pcm_gemm_kernel<64, 1, NARROW>;
+    case 96: return pcm_gemm_kernel<96, 1, NARROW>;
+    case 128: return pcm_gemm_kernel<128, 1, NARROW>;
+    case 160: return pcm_gemm_kernel<160, 1, NARROW>;
+    case 192: return pcm_gemm_kernel<192, 1, NARROW>;
+    case 224: return pcm_gemm_kernel<224, 1, NARROW>;
+    default: return pcm_gemm_kernel<256, 1, NARROW>;
   }
 }
 
@@ -491,6 +515,36 @@ static int gemm_ksplit(const pcm_gemm_desc* d) {
   const int ks = d->ksplit < nkb ? d->ksplit : nkb;
   const int per = (nkb + ks - 1) / ks;
   return (nkb + per - 1) / per;
+}
+
+// Rows of A source a_src: an A source with fewer rows than the output only feeds the leading M tiles (TMA
+// would zero fill the rest: the kernel skips those K blocks instead).  Whole 128-row tiles only, unsplit
+// launches only; 0 = the entry applies to every row.
+static int gemm_entry_m_hi(const pcm_gemm_desc* d, const pcm_kentry& k) {
+  const pcm_asrc& a = d->a[k.a_src];
+  const long long rows = d->lin ? a.W : static_cast<long long>(a.B) * d->geoW * d->geoH;
+  return rows < d->M && rows % 128 == 0 && d->ksplit <= 1 ? static_cast<int>(rows) : 0;
+}
+
+// Rows of an output tile: 256 (two 128-row slabs against each weight tile in shared memory: 27 % fewer
+// operand bytes per FLOP at BN = 160) for BN 128 / 160 launches that run unsplit, whose every tile runs at
+// least kTallMinKBlocks K blocks, whose M-ranged entries end on 256-row boundaries, and whose 256-row tiles
+// take at most half as many waves of the persistent grid as 128-row tiles (a 256-row tile runs twice as
+// long: fewer waves must not mean more time).  Short K loops lose: with 4 stages instead of 5 and twice the
+// epilogue per tile, a 6- or 11-block Linear ran 3-4 % slower on 256-row tiles, 45-block convolutions
+// 4-8 % faster (H100 SXM, DESIGN 3.1).  One rule for the launch and pcm_gemm_plan_rows.
+constexpr int kTallMinKBlocks = 32;
+static int gemm_plan_rows(const pcm_gemm_desc* d) {
+  if ((d->block_n != 128 && d->block_n != 160) || gemm_ksplit(d) != 1) return 128;
+  int nkb = 0;   // K blocks of the entries every tile runs (N-ranged ones feed some tiles only)
+  for (int e = 0; e < d->num_prog; ++e) {
+    if (gemm_entry_m_hi(d, d->prog[e]) % 256 != 0) return 128;
+    if (d->prog[e].n_hi == 0 && gemm_entry_m_hi(d, d->prog[e]) == 0) nkb += d->prog[e].nchunks;
+  }
+  if (nkb < kTallMinKBlocks) return 128;
+  const long long tn = (d->N + d->block_n - 1) / d->block_n, sms = num_sms();
+  const long long t128 = (d->M + 127) / 128 * tn, t256 = (d->M + 255) / 256 * tn;
+  return 2 * ((t256 + sms - 1) / sms) <= (t128 + sms - 1) / sms ? 256 : 128;
 }
 
 static int validate_gemm(const pcm_gemm_desc* d) {
@@ -592,16 +646,9 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
     const int a_left = d->a[k.a_src].C - k.a_c0, b_left = d->b[k.b_src].K - k.b_k0;
     const int kend = a_left < b_left ? a_left : b_left;
     if (kend < 64 * k.nchunks) narrow = true;
-    p.prog[e] = KEntry{k.a_src, k.b_src, k.dw, k.dh, k.nchunks, k.a_c0, k.b_k0, k.n_lo, k.n_hi, 0, kend};
-    {  // an A source with fewer rows than the output only feeds the leading M tiles (TMA would zero
-       // fill the rest: skip those K blocks instead); whole tiles only
-      const pcm_asrc& a = d->a[k.a_src];
-      const long long rows = d->lin ? a.W : static_cast<long long>(a.B) * d->geoW * d->geoH;
-      if (rows < d->M && rows % 128 == 0 && d->ksplit <= 1) {
-        p.prog[e].m_hi = static_cast<int>(rows);
-        p.filtered = 1;
-      }
-    }
+    p.prog[e] = KEntry{k.a_src, k.b_src, k.dw, k.dh, k.nchunks, k.a_c0, k.b_k0, k.n_lo, k.n_hi,
+                       gemm_entry_m_hi(d, k), kend};
+    if (p.prog[e].m_hi != 0) p.filtered = 1;
     nkb += k.nchunks;
     if (k.n_hi != 0) {
       if (k.n_lo % d->block_n != 0 || (k.n_hi % d->block_n != 0 && k.n_hi < d->N) || k.n_hi <= k.n_lo)
@@ -616,10 +663,11 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
   p.geoW = d->lin ? 1 : d->geoW;
   p.geoHW = d->lin ? 1 : d->geoW * d->geoH;
   p.block_n = d->block_n;
-  p.tiles_m = (d->M + 127) / 128;
+  const int rows = gemm_plan_rows(d);
+  p.tiles_m = (d->M + rows - 1) / rows;
   p.tiles_n = (d->N + d->block_n - 1) / d->block_n;
   p.num_kblocks = nkb;
-  const int stage_bytes = kATileBytes + d->block_n * 128;
+  const int stage_bytes = rows / 128 * kATileBytes + d->block_n * 128;
   int S = (kSmemLimit - 1024 - kStagingBytes) / stage_bytes;
   if (S > kMaxStages) S = kMaxStages;
   if (S < 2) return set_error("pcm_gemm: tile too large for shared memory");
@@ -641,11 +689,12 @@ static int launch_gemm(const pcm_gemm_desc* d, cudaStream_t stream) {
   p.ksplit = gemm_ksplit(d);   // (m_hi is only set for ksplit <= 1, so a split program is never filtered)
 
   const size_t smem = static_cast<size_t>(S) * stage_bytes + kStagingBytes + 1024;
-  const GemmKernel kernel = narrow ? gemm_kernel_for<true>(d->block_n) : gemm_kernel_for<false>(d->block_n);
-  static bool attr_set[2][9] = {};
-  if (!attr_set[narrow][d->block_n / 32]) {
+  const GemmKernel kernel =
+      narrow ? gemm_kernel_for<true>(d->block_n, rows) : gemm_kernel_for<false>(d->block_n, rows);
+  static bool attr_set[2][2][9] = {};
+  if (!attr_set[rows / 256][narrow][d->block_n / 32]) {
     CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-    attr_set[narrow][d->block_n / 32] = true;
+    attr_set[rows / 256][narrow][d->block_n / 32] = true;
   }
   if (d->dep_a_src1 > 0 && p.ksplit == 1) {  // (split-K: the finalize kernel follows; keep the plain chain)
     p.dep_a_map = d->dep_a_src1 - 1;
@@ -731,6 +780,7 @@ extern "C" int pcm_gemm(const pcm_gemm_desc* d, void* stream) {
   return pcm::launch_gemm(d, reinterpret_cast<cudaStream_t>(stream));
 }
 extern "C" int pcm_gemm_check(const pcm_gemm_desc* d) { return pcm::validate_gemm(d); }
+extern "C" int pcm_gemm_plan_rows(const pcm_gemm_desc* d) { return pcm::gemm_plan_rows(d); }
 extern "C" int pcm_wgrad_check(const pcm_wgrad_desc* d) { return pcm::validate_wgrad(d); }
 extern "C" int pcm_wgrad(const pcm_wgrad_desc* d, void* stream) {
   return pcm::launch_wgrad(d, reinterpret_cast<cudaStream_t>(stream));

@@ -22,6 +22,7 @@ SHAPES = [  # (kind, M|(B,H,W), K|Cin, N, residual)
     ("lin", 98304, 384, 320, True),
     ("lin", 98304, 384, 2560, False),
     ("lin", 24576, 704, 640, True),
+    ("conv", (24, 64, 64), 320, 320, True),
 ]
 sel = [int(a) for a in sys.argv[1:]] or range(len(SHAPES))
 iters = int(os.environ.get("ITERS", "20"))
