@@ -120,7 +120,8 @@ const char* pcm_last_error(void);
 int pcm_version(void);
 int pcm_num_sms(void);
 
-/* wgmma implicit GEMM / conv and LoRA wgrad.  A descriptor the kernels cannot serve is rejected on the
+/* wgmma implicit GEMM / conv and LoRA wgrad.  Conv mode takes images whose width divides 128 or is a multiple
+ * of 128 (pcm_wgrad: divides 128).  A descriptor the kernels cannot serve is rejected on the
  * host before any CUDA call, pcm_last_error() naming the field: M, N < 1, a null out, conv mode with geoW,
  * geoH, epiW or epiHW < 1, and alignment.  A launch with a bf16 output, no activation and no K split
  * actually run (ksplit <= 1, N-ranged entries, or a program too short to split: ksplit is capped at one
@@ -196,6 +197,31 @@ int pcm_timestep_embed(const int64_t* t, int B, int C, void* out, void* stream);
 int pcm_colsum(const void* x, int B, int HW, int C, void* out, void* stream);
 int pcm_add_bf16(const void* a, const void* b, int64_t n, void* out, void* stream);
 int pcm_cast_f32_bf16(const float* in, int64_t n, void* out, void* stream);
+
+/* ---- Stable Diffusion VAE (AutoencoderKL) glue around pcm_gemm ---------------------------
+ * Replaces, in diffusers' AutoencoderKL (vae.encode(pixels).latent_dist.sample(), T15:1127-1136, and the
+ * validation pipeline's vae.decode): the mid-block attention's softmax, DiagonalGaussianDistribution,
+ * post_quant_conv and the image postprocessing.
+ * pcm_softmax_rows: p[r, :] = bf16(softmax(s[r, :])) with fp32 max and sum, s fp32 [rows, cols] (row stride lds,
+ *   16-byte aligned), p bf16 (row stride ldp, 8-byte aligned); cols, lds, ldp multiples of 4.
+ * pcm_transpose_bf16: out[b][c][r] = in[b][r][c] for batch bf16 [rows, cols] matrices; ldi / ldo row strides,
+ *   bsi / bso batch strides (elements).
+ * pcm_latent_dist: quant_conv (1x1, 8 -> 8; w bf16 [8][8], bias fp32 [8]) on h fp32 NHWC [B*HW, 8] (inputs and
+ *   result rounded to bf16), then mean = moments[:4], logvar = clamp(moments[4:], -30, 20), std = exp(logvar / 2),
+ *   written fp32 NCHW [B, 4, HW].  noise (fp32 NCHW [B, 4, HW]) or NULL: sample = (mean + std * noise) * scale,
+ *   each operation rounded on its own.
+ * pcm_vae_dec_in: post_quant_conv (1x1, 4 -> 4; w bf16 [4][4], bias fp32 [4]) on bf16(z / div), z fp32 NHWC [M, 4];
+ *   out bf16 NHWC [M, 8]: the result in channels 0..3, zeros in 4..7 (the A source of the decoder's conv_in on
+ *   pcm_gemm).  z, out 16-byte aligned.
+ * pcm_image_exit: v = clamp(x / 2 + 0.5, 0, 1) for x fp32 NHWC [B, HW, C]; out (may be NULL) fp32 NCHW, u8 (may be
+ *   NULL) uint8 NHWC round(255 v), round half to even. */
+int pcm_softmax_rows(const float* s, int64_t rows, int cols, int64_t lds, void* p, int64_t ldp, void* stream);
+int pcm_transpose_bf16(const void* in, int rows, int cols, int64_t ldi, int64_t bsi, int batch, void* out,
+                       int64_t ldo, int64_t bso, void* stream);
+int pcm_latent_dist(const float* h, int B, int HW, const void* w, const float* bias, const float* noise,
+                    float scale, float* mean, float* logvar, float* std, float* sample, void* stream);
+int pcm_vae_dec_in(const float* z, int64_t M, const void* w, const float* bias, float div, void* out, void* stream);
+int pcm_image_exit(const float* x, int B, int HW, int C, float* out, void* u8, void* stream);
 
 /* ---- PCM solver arithmetic (fused; fp32 latents, batch outermost, `per` elements/sample) ---
  * coef: [B, 16] doubles (internal layout, see csrc/pcm_ops.cu). */

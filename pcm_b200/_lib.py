@@ -118,6 +118,11 @@ EXPORTS = [
     "pcm_lora_refresh",
     "pcm_lora_fuse",
     "pcm_sample_step",
+    "pcm_softmax_rows",
+    "pcm_transpose_bf16",
+    "pcm_latent_dist",
+    "pcm_vae_dec_in",
+    "pcm_image_exit",
 ]
 
 
@@ -159,6 +164,11 @@ ARGTYPES = {
     "pcm_lora_refresh": [P, P, I, L64, F, P, P],
     "pcm_lora_fuse": [P, P, I, L64, F, P],
     "pcm_sample_step": [P, P, P, P, L64, I, I, P, D, D, D, D, I, P],
+    "pcm_softmax_rows": [P, L64, I, L64, P, L64, P],
+    "pcm_transpose_bf16": [P, I, I, L64, L64, I, P, L64, L64, P],
+    "pcm_latent_dist": [P, I, I, P, P, P, F, P, P, P, P, P],
+    "pcm_vae_dec_in": [P, L64, P, P, F, P, P],
+    "pcm_image_exit": [P, I, I, I, P, P, P],
 }
 
 

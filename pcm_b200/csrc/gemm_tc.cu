@@ -108,12 +108,16 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
         const int tn = tile - tm * p.tiles_n;
         if (p.dep_a_map >= 0) tm = p.tiles_m - 1 - tm;  // adapter-free rows first (see dep_a_src1)
         const int m0 = tm * kRows, n0 = tn * BN;
-        int b0[MS] = {}, h0[MS] = {};   // conv mode: TMA coordinates of each 128-row slab
+        // conv mode: TMA coordinates of each 128-row slab (w0 = 0 unless W is a multiple of 128 and the
+        // slab is one 128-pixel run of an image row)
+        int b0[MS] = {}, h0[MS] = {}, w0[MS] = {};
         if (!p.lin) {
 #pragma unroll
           for (int s = 0; s < MS; ++s) {
             b0[s] = (m0 + 128 * s) / p.geoHW;
-            h0[s] = (m0 + 128 * s - b0[s] * p.geoHW) / p.geoW;
+            const int r = m0 + 128 * s - b0[s] * p.geoHW;
+            h0[s] = r / p.geoW;
+            w0[s] = r - h0[s] * p.geoW;
           }
         }
         int kidx = 0;
@@ -145,7 +149,7 @@ pcm_gemm_kernel(const __grid_constant__ GemmParams p) {
                             m0 + 128 * s, 0, 0);
               else
                 tma_load_4d(sa + s * kATileBytes, &p.a_maps[en.a_map], &full_bar[stage], en.a_c0 + c * 64,
-                            en.dw, h0[s] + en.dh, b0[s]);
+                            w0[s] + en.dw, h0[s] + en.dh, b0[s]);
             }
             if ((p.b_blocked >> en.b_map) & 1)   // K-blocked weights: (64, N, K/64) view, contiguous tile
               tma_load_3d(sb, &p.b_maps[en.b_map], &full_bar[stage], 0, n0, (en.b_k0 >> 6) + c);
@@ -463,8 +467,14 @@ static int encode_asrc(CUtensorMap* map, const pcm_asrc& a, int lin, int geoW, i
   } else {
     dims[0] = a.C; dims[1] = a.W; dims[2] = a.H; dims[3] = a.B;
     strides[0] = a.sW * 2; strides[1] = a.sH * 2; strides[2] = a.sB * 2;
+    // W dividing 128: a box of whole image rows (and images); W a multiple of 128: a box of 128 pixels of
+    // one row, placed at the tile's w0 by the producer
+    if (geoW % 128 == 0) {
+      box[0] = box_c; box[1] = 128; box[2] = 1; box[3] = 1;
+      return encode_tmap(map, a.ptr, 4, dims, strides, box, estr);
+    }
     const int bw = geoW;
-    if (bw > 128 || 128 % bw != 0) return set_error("conv geometry: W must divide 128");
+    if (bw > 128 || 128 % bw != 0) return set_error("conv geometry: W must divide 128 or be a multiple of 128");
     int bh = 128 / bw;
     if (bh > geoH) bh = geoH;
     int bb = 128 / (bw * bh);
@@ -595,6 +605,7 @@ static int validate_wgrad(const pcm_wgrad_desc* d) {
   if (d->os_col == 0) return set_error("pcm_wgrad: os_col is zero");
   if (d->num_taps < 1 || d->num_taps > 9) return set_error("pcm_wgrad: bad tap count");
   if (!d->lin && (d->geoW < 1 || d->geoH < 1)) return set_error("pcm_wgrad: geoW and geoH must be >= 1 in conv mode");
+  if (!d->lin && d->geoW > 128) return set_error("pcm_wgrad: conv geometry: W must divide 128");
   const int qw = d->q.C - d->q_c0 < 64 ? d->q.C - d->q_c0 : 64;
   if (d->q_c0 < 0 || qw < 8 || qw % 8 != 0)
     return set_error("pcm_wgrad: the rank slice q[:, q_c0:] must hold a positive multiple of 8 columns");

@@ -380,6 +380,51 @@ def conv3x3_c4(x, w, bias, out, sgn=1, round_in=True):
     return out
 
 
+def softmax_rows(s, p):
+    """p = bf16(softmax(s, -1)), fp32 max and sum: s fp32 [rows, cols], p bf16 [rows, cols] (row strides free)."""
+    assert s.dtype == torch.float32 and p.dtype == BF16 and s.shape == p.shape and s.stride(1) == p.stride(1) == 1
+    _call("pcm_softmax_rows", _p(s), s.shape[0], s.shape[1], s.stride(0), _p(p), p.stride(0))
+    return p
+
+
+def transpose_bf16(x, out):
+    """out[b] = x[b]^T for bf16 [batch, rows, cols] -> [batch, cols, rows] (row and batch strides free)."""
+    assert x.dtype == out.dtype == BF16 and x.stride(2) == out.stride(2) == 1
+    batch, rows, cols = x.shape
+    assert tuple(out.shape) == (batch, cols, rows)
+    _call("pcm_transpose_bf16", _p(x), rows, cols, x.stride(1), x.stride(0), batch, _p(out), out.stride(1),
+          out.stride(0))
+    return out
+
+
+def latent_dist(h, w, bias, noise, scale, mean, logvar, std, sample):
+    """quant_conv + DiagonalGaussianDistribution: h fp32 [B, hh, ww, 8]; mean / logvar / std (/ sample with
+    noise) fp32 NCHW [B, 4, hh, ww]."""
+    B, hh, ww, eight = h.shape
+    assert eight == 8 and h.dtype == torch.float32 and h.is_contiguous() and mean.is_contiguous()
+    assert noise is None or (noise.is_contiguous() and noise.shape == mean.shape)
+    _call("pcm_latent_dist", _p(h), B, hh * ww, _p(w), _p(bias), _p(noise), scale, _p(mean), _p(logvar), _p(std),
+          _p(sample))
+
+
+def vae_dec_in(z, w, bias, div, out):
+    """post_quant_conv on z / div: z fp32 NHWC [B, h, w, 4] -> out bf16 NHWC [B, h, w, 8], channels 4..7 zero."""
+    assert z.dtype == torch.float32 and out.dtype == BF16 and z.is_contiguous() and out.is_contiguous()
+    assert z.shape[-1] == 4 and tuple(out.shape) == tuple(z.shape[:-1]) + (8,)
+    _call("pcm_vae_dec_in", _p(z), z.numel() // 4, _p(w), _p(bias), div, _p(out))
+    return out
+
+
+def image_exit(x, out, u8=None):
+    """(x / 2 + 0.5).clamp(0, 1): x fp32 NHWC [B, H, W, C] -> out fp32 NCHW (or None), u8 uint8 NHWC (or None)."""
+    B, H, W, Cc = x.shape
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    assert out is None or (out.is_contiguous() and tuple(out.shape) == (B, Cc, H, W))
+    assert u8 is None or (u8.dtype == torch.uint8 and u8.is_contiguous() and u8.shape == x.shape)
+    _call("pcm_image_exit", _p(x), B, H * W, Cc, _p(out), _p(u8))
+    return out
+
+
 def timestep_embed(t, out):
     _call("pcm_timestep_embed", _p(t), out.shape[0], out.shape[1], _p(out))
     return out

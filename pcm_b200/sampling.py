@@ -3,15 +3,16 @@
 What the reference's validation (train_pcm_lora_sd15.py:120-207, log_validation) runs after training
 steps: a StableDiffusionPipeline with DDIMScheduler(timestep_spacing="trailing", clip_sample=False,
 set_alpha_to_one=False), the LoRA fused into the UNet (`pipeline.fuse_lora()`), classifier-free guidance
-when guidance_scale > 1, eta = 0.  VAE decoding and CLIP encoding stay outside: the sampler takes prompt
-embeddings and returns the latents the pipeline hands to `vae.decode` (before the 1 / scaling_factor
-scale).
+when guidance_scale > 1, eta = 0.  CLIP encoding stays outside: the sampler takes prompt embeddings and
+returns the latents the pipeline hands to `vae.decode` (before the 1 / scaling_factor scale), or, given a
+pcm_b200.vae.AutoencoderKL, the decoded images (output_type "pt" / "pil").
 
   * the UNet is an inference copy of the trained network (UNetB200.fused_inference_net): the LoRA targets'
     frozen weights are fused copies W + s B A (pcm_lora_fuse, one launch), every other tensor is shared;
   * each step is n UNet forwards at batch B (or 2B = [uncond; cond] with guidance) and one pcm_sample_step
     launch (CFG mix + DDIM update);
-  * on CUDA the whole loop of one shape is captured into a CUDA graph on first use and replayed.
+  * on CUDA the whole loop of one shape is captured into a CUDA graph on first use and replayed, with the
+    VAE decode and the image postprocessing in the same graph when images are asked for.
 """
 import math
 import os
@@ -76,10 +77,11 @@ class PCMSampler:
     sampler.fuse()      # after more training: fuse the current LoRA masters again
     """
 
-    def __init__(self, unet, *, alphas_cumprod=None, prediction_type="epsilon"):
+    def __init__(self, unet, *, alphas_cumprod=None, prediction_type="epsilon", vae=None):
+        """vae: a pcm_b200.vae.AutoencoderKL for output_type "pt" / "pil" (None: latents only)."""
         if prediction_type not in ("epsilon", "v_prediction"):
             raise ValueError(f"Prediction type {prediction_type} currently not supported.")
-        self.unet, self.cfg, self.dev = unet, unet.cfg, unet.dev
+        self.unet, self.cfg, self.dev, self.vae = unet, unet.cfg, unet.dev, vae
         self.pred_type = 0 if prediction_type == "epsilon" else 1
         acp = sd15_alphas_cumprod() if alphas_cumprod is None else alphas_cumprod
         self.alphas_cumprod = acp.detach().float().cpu()
@@ -146,7 +148,7 @@ class PCMSampler:
         plan = self._plans.get(key)
         if plan is not None:
             return plan
-        B, h, w, n, cfg_on, S = key
+        B, h, w, n, cfg_on, S, images = key
         nb = 2 if cfg_on else 1
         dev, cfg = self.dev, self.cfg
         plan = types.SimpleNamespace(B=B, nb=nb, S=S, cfg_on=cfg_on, graph=None)
@@ -160,6 +162,10 @@ class PCMSampler:
                           torch.zeros(nb * B, cfg.num_time_ids, device=dev, dtype=torch.int64))
         plan.coef = step_coefficients(self.alphas_cumprod, n)
         plan.ts = torch.tensor([[c[0]] * (nb * B) for c in plan.coef], dtype=torch.int64).to(dev)
+        plan.img = plan.u8 = None
+        if images:      # [0, 1] NCHW fp32 and uint8 NHWC images of the decoded latents
+            plan.img = torch.zeros(B, 3, 8 * h, 8 * w, device=dev, dtype=torch.float32)
+            plan.u8 = torch.zeros(B, 8 * h, 8 * w, 3, device=dev, dtype=torch.uint8)
         self._plans[key] = plan
         return plan
 
@@ -171,27 +177,40 @@ class PCMSampler:
         for i, (_, sa, ss, sap, ssp) in enumerate(plan.coef):
             eps = self.net.forward(plan.lat, plan.ts[i], plan.ctx, lora=False, added_cond=plan.added)
             ops.sample_step(eps, x, x, x2, plan.g, sa, ss, sap, ssp, self.pred_type)
+        if plan.img is not None:    # the pipeline's vae.decode(latents / scaling_factor) and postprocess
+            self.vae.decode_images(x, self.vae.config.scaling_factor, plan.img, plan.u8)
 
     def _hold_workspaces(self):
         ws = ops._GN_WS.get(torch.device(self.dev))
         if ws is not None and all(ws is not h for h in self._held):
             self._held.append(ws)
+        if self.vae is not None:
+            self.vae._hold_workspaces()
 
     def __call__(self, prompt_embeds, negative_prompt_embeds=None, *, num_inference_steps, guidance_scale=1.0,
                  num_images_per_prompt=1, height, width, latents=None, generator=None, text_embeds=None,
-                 time_ids=None, negative_text_embeds=None):
-        """Returns fp32 NCHW latents [P * num_images_per_prompt, 4, height / 8, width / 8].  Images of one
+                 time_ids=None, negative_text_embeds=None, output_type="latent"):
+        """output_type "latent" (default): fp32 NCHW latents [P * num_images_per_prompt, 4, height / 8, width / 8];
+        "pt": the decoded fp32 NCHW images in [0, 1] [P * num_images_per_prompt, 3, height, width]; "pil": those
+        images as a list of PIL images.  Images of one
         prompt are consecutive (diffusers' `repeat` of the embeddings); with guidance_scale > 1 the UNet runs
         the pipeline's [uncond; cond] batch.  `latents`: the initial noise (default: randn from
         `generator`, init_noise_sigma = 1)."""
         n, g, nipp = num_inference_steps, float(guidance_scale), num_images_per_prompt
+        if output_type not in ("latent", "pt", "pil"):
+            raise ValueError(f"output_type must be 'latent', 'pt' or 'pil', got {output_type!r}")
+        images = output_type != "latent"
+        if images and self.vae is None:
+            raise ValueError(f"output_type {output_type!r} needs the sampler built with vae=AutoencoderKL(...)")
         P, B, h, w, cfg_on = self._check(prompt_embeds, negative_prompt_embeds, n, g, nipp, height, width,
                                          latents, text_embeds, time_ids, negative_text_embeds)
         cfg = self.cfg
         if latents is None:
             gdev = generator.device if generator is not None else torch.device(self.dev)
             latents = torch.randn(B, cfg.in_channels, h, w, generator=generator, device=gdev, dtype=torch.float32)
-        plan = self._plan((B, h, w, int(n), cfg_on, prompt_embeds.shape[1]))
+        if images:
+            self.vae._check_size(height, width, "decode")
+        plan = self._plan((B, h, w, int(n), cfg_on, prompt_embeds.shape[1], images))
 
         def rep(t):
             return t.repeat_interleave(nipp, 0)
@@ -232,4 +251,9 @@ class PCMSampler:
                     self._run(plan)
             load()
             plan.graph.replay()
+        if output_type == "pt":
+            return plan.img.clone()
+        if output_type == "pil":
+            from PIL import Image
+            return [Image.fromarray(a) for a in plan.u8.cpu().numpy()]
         return plan.lat[:B].permute(0, 3, 1, 2).contiguous()

@@ -104,6 +104,10 @@ def parse_args(argv=None, extra=None):
                    help=".pt dict {prompt_embeds [P,77,D]} (+ text_embeds [P,*], time_ids [P or 1,6] for SDXL): "
                         "sample 4 images per prompt in --multiphase steps every --validation_steps (T15:1345-1365) "
                         "into output_dir/validation/step-N/cfg-{g}.pt")
+    p.add_argument("--validation_images", action="store_true",
+                   help="with --validation_prompt_embeds: also decode each validation image with the VAE (from "
+                        "--pretrained_vae_model_name_or_path, else <pretrained_teacher_model>/vae, else a seeded "
+                        "random SD1.5 VAE under --synthetic) into output_dir/validation/step-N/cfg-{g}/NNNN.png")
     args = p.parse_args(argv)
     env_local_rank = int(os.environ.get("LOCAL_RANK", -1))   # same override as the reference
     if env_local_rank != -1 and env_local_rank != args.local_rank:
@@ -211,6 +215,31 @@ class _Validation:
         if any(g > 1 for g in self.guidances) and self.ne is None:
             raise SystemExit("validation with guidance > 1 needs the empty-prompt embedding (--uncond_embeds)")
         self.sampler = None
+        self.vae = None
+        if args.validation_images:
+            from .vae import AutoencoderKL
+            if args.pretrained_vae_model_name_or_path:
+                self.vae = AutoencoderKL.from_pretrained(args.pretrained_vae_model_name_or_path, subfolder=None,
+                                                         device=st.unet.dev)
+            elif args.pretrained_teacher_model:
+                self.vae = AutoencoderKL.from_pretrained(args.pretrained_teacher_model, subfolder="vae",
+                                                         device=st.unet.dev)
+            elif args.synthetic:
+                self.vae = AutoencoderKL.from_pretrained(None, device=st.unet.dev, seed=args.seed or 0)
+            else:
+                raise SystemExit("--validation_images needs a VAE: --pretrained_vae_model_name_or_path or "
+                                 "--pretrained_teacher_model")
+
+    def _save_images(self, lats, out_dir, g):
+        """One PNG per validation image: the pipeline's vae.decode(latents / scaling_factor), postprocessed."""
+        from PIL import Image
+        d = os.path.join(out_dir, f"cfg-{g}")
+        os.makedirs(d, exist_ok=True)
+        z = lats.permute(0, 2, 3, 1).contiguous()
+        u8 = torch.empty(z.shape[0], 8 * z.shape[1], 8 * z.shape[2], 3, device=z.device, dtype=torch.uint8)
+        self.vae.decode_images(z, self.vae.config.scaling_factor, None, u8)
+        for i, a in enumerate(u8.cpu().numpy()):
+            Image.fromarray(a).save(os.path.join(d, f"{i:04d}.png"))
 
     def __call__(self, global_step):
         from .sampling import PCMSampler
@@ -237,6 +266,8 @@ class _Validation:
                                          num_images_per_prompt=4, height=res, width=res, generator=gen, **ex))
             torch.save({"latents": torch.cat(lats).cpu(), "seed": seed, "guidance_scale": g},
                        os.path.join(out_dir, f"cfg-{g}.pt"))
+            if self.vae is not None:
+                self._save_images(torch.cat(lats), out_dir, g)
 
 
 def main(args):

@@ -33,6 +33,32 @@ _S2 = ((1, -1), (0, 0), (1, 0))
 _S2_PLANE = [[(k, sh) for k, (par, sh) in enumerate(_S2) if par == p] for p in range(2)]
 
 
+def conv_prog(xs, k, stride, cin_total, s2=_S2):
+    """(a_srcs, prog) of a k x k convolution over channel-concatenated NHWC sources xs.  A stride-2 3x3
+    convolution reads the four parity planes of xs[0]; s2 maps its kernel index to (input parity, shift in
+    the parity plane): the default is pad 1 (the UNet's downsamplers)."""
+    if stride == 2:
+        x = xs[0]
+        planes = [x[:, p::2, q::2, :] for p in range(2) for q in range(2)]
+        srcs = [ops.asrc_nhwc(pl) for pl in planes]
+        prog = []
+        for kh in range(3):
+            for kw in range(3):
+                p, dh = s2[kh]
+                q, dw = s2[kw]
+                prog.append((p * 2 + q, 0, dw, dh, cin_total // 64, 0, (kh * 3 + kw) * cin_total))
+        return srcs, prog
+    srcs = [ops.asrc_nhwc(x) for x in xs]
+    taps = TAPS3 if k == 3 else [(0, 0)]
+    prog, coff = [], 0
+    for si, x in enumerate(xs):
+        ci = x.shape[-1]
+        for t, (dw, dh) in enumerate(taps):
+            prog.append((si, 0, dw, dh, ci // 64, 0, t * cin_total + coff))
+        coff += ci
+    return srcs, prog
+
+
 # tape records: what the backward of one op needs (views of the LoRA samples' rows only).  `op` names the
 # op kind; T is the layer's LoRA down-projection x A^T (None: no adapter).
 LinearRec = namedtuple("LinearRec", "op name xs T")
@@ -581,29 +607,6 @@ class UNetB200:
     def _new(self, *shape, dtype=BF16):
         return torch.empty(*shape, device=self.dev, dtype=dtype)
 
-    def _conv_prog(self, xs, k, stride, cin_total):
-        """(a_srcs, prog) of a k x k convolution over channel-concatenated sources xs."""
-        if stride == 2:
-            x = xs[0]
-            planes = [x[:, p::2, q::2, :] for p in range(2) for q in range(2)]
-            srcs = [ops.asrc_nhwc(pl) for pl in planes]
-            prog = []
-            for kh in range(3):
-                for kw in range(3):
-                    p, dh = _S2[kh]
-                    q, dw = _S2[kw]
-                    prog.append((p * 2 + q, 0, dw, dh, cin_total // 64, 0, (kh * 3 + kw) * cin_total))
-            return srcs, prog
-        srcs = [ops.asrc_nhwc(x) for x in xs]
-        taps = TAPS3 if k == 3 else [(0, 0)]
-        prog, coff = [], 0
-        for si, x in enumerate(xs):
-            ci = x.shape[-1]
-            for t, (dw, dh) in enumerate(taps):
-                prog.append((si, 0, dw, dh, ci // 64, 0, t * cin_total + coff))
-            coff += ci
-        return srcs, prog
-
     def conv3(self, P, name, xs, stride=1, rowvec=None, residual=None, out_fp32=False, save=None):
         """3x3 pad-1 convolution (+LoRA) over NHWC sources xs (channel concat), fused epilogue; appends its
         ConvRec to the list `save`."""
@@ -611,7 +614,7 @@ class UNetB200:
         B, H, W, _ = xs[0].shape
         Ho, Wo = H // stride, W // stride
         M, N = B * Ho * Wo, L.cout
-        srcs, prog = self._conv_prog(xs, 3, stride, L.cin)
+        srcs, prog = conv_prog(xs, 3, stride, L.cin)
         bs = [ops.bsrc(self.operands[name].w)]
         T = None
         lbn = P.rows(B)   # samples that carry the LoRA adapter (the leading ones of the batch)
@@ -619,7 +622,7 @@ class UNetB200:
         if P.lora and L.lora is not None:
             # T = A(x) only for the LoRA samples; the other samples see T rows that TMA zero-fills
             T = self._new(lbn, Ho, Wo, self.r)
-            srcs_l, prog_l = (srcs, prog) if lbn == B else self._conv_prog(xl, 3, stride, L.cin)
+            srcs_l, prog_l = (srcs, prog) if lbn == B else conv_prog(xl, 3, stride, L.cin)
             ops.gemm(srcs_l, [ops.bsrc(L.lora.a_fwd)], prog_l, lin=False, M=lbn * Ho * Wo, N=self.r,
                      geo=(Wo, Ho), out=T.view(lbn * Ho * Wo, self.r))
             prog = prog + [(len(srcs), 1, 0, 0, self.rc, 0, 0)]
