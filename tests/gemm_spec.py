@@ -320,22 +320,25 @@ def _silu(x):
     return x * torch.sigmoid(x)
 
 
-def reference(spec, T, desc=None, row_block=16384):
+def reference(spec, T, desc=None, row_block=16384, rows=None):
     """(ref, S, base) of one pcm_gemm launch, each [M, N]: the float64 result, the same sum over absolute
     values (alpha |A| |B|^T + |bias| + |rowvec| + |residual|), and a torch baseline with the kernel's
     roundings (bf16 operands, fp32 accumulate, fp32 epilogue) before its one output rounding.
     Written from include/pcm_b200.h: entry e multiplies min(64 nchunks, a.C - a_c0, b.K - b_k0) K columns
-    of source pixel (b, h + dh, w + dw), zero outside the source, against rows [n_lo, n_hi) of b."""
+    of source pixel (b, h + dh, w + dw), zero outside the source, against rows [n_lo, n_hi) of b.
+    rows = (m0, m1): only output rows m0 .. m1 - 1 ([m1 - m0, N] results), for launches too large to hold
+    in float64 at once."""
     d = desc or spec["desc"]
     dev = T.device
     M, N = d["M"], d["N"]
-    ref = torch.empty(M, N, dtype=torch.float64, device=dev)
-    S, base = torch.empty_like(ref), torch.empty(M, N, dtype=torch.float32, device=dev)
+    m0, m1 = rows or (0, M)
+    ref = torch.empty(m1 - m0, N, dtype=torch.float64, device=dev)
+    S, base = torch.empty_like(ref), torch.empty(m1 - m0, N, dtype=torch.float32, device=dev)
     off, bimg = _row_offsets(M, d["epiW"], d["epiHW"], d["osW"], d["osH"], d["osB"])
     off, bimg = off.to(dev), bimg.to(dev)
     al = float(d["alpha"])
-    for r0 in range(0, M, row_block):
-        m = torch.arange(r0, min(M, r0 + row_block), device=dev)
+    for r0 in range(m0, m1, row_block):
+        m = torch.arange(r0, min(m1, r0 + row_block), device=dev)
         acc = torch.zeros(len(m), N, dtype=torch.float64, device=dev)
         ab, a32 = torch.zeros_like(acc), torch.zeros(len(m), N, dtype=torch.float32, device=dev)
         for e in d["prog"]:
@@ -365,7 +368,7 @@ def reference(spec, T, desc=None, row_block=16384):
             acc, a32 = _silu(acc), _silu(a32)
         else:
             assert d["act"] == 0
-        ref[m], S[m], base[m] = acc, ab, a32
+        ref[m - m0], S[m - m0], base[m - m0] = acc, ab, a32
     return ref, S, base
 
 

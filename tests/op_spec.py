@@ -1,5 +1,5 @@
 """Pointer-free launch specs of the normalisation, glue and optimiser kernels (csrc/norm.cu, elementwise.cu,
-optim.cu), a float64 reference for each and a derived elementwise error bound.  Test infrastructure: nothing
+optim.cu, and the VAE's glue in vae.cu), a float64 reference for each and a derived elementwise error bound.  Test infrastructure: nothing
 under pcm_b200/ imports it.
 
 A spec is plain data: the op name, its arguments as `ops._call` passed them (scalars as they are, pointers as
@@ -15,6 +15,7 @@ reference runs on any torch device, so the checker itself is tested on the CPU (
 import contextlib
 import copy
 import ctypes
+import functools
 import json
 import math
 
@@ -45,6 +46,11 @@ ARGS = {
     "pcm_adamw_clip": "p g m v n state beta1 beta2 eps wd max_norm inv_world sumsq zero_grad",
     "pcm_ema_update": "targ src n rate",
     "pcm_lora_refresh": "master table num_entries total_work scale opnd",
+    "pcm_softmax_rows": "s rows cols lds p ldp",
+    "pcm_transpose_bf16": "in rows cols ldi bsi batch out ldo bso",
+    "pcm_latent_dist": "h B HW w bias noise scale mean logvar std sample",
+    "pcm_vae_dec_in": "z M w bias div out",
+    "pcm_image_exit": "x B HW C out u8",
 }
 ARGS = {k: v.split() for k, v in ARGS.items()}
 # `_call` entry points with suites of their own: attention (test_attn_*), the PCM solver arithmetic
@@ -62,7 +68,9 @@ _OUTS = {
     "pcm_upsample2x_fwd": ("out",), "pcm_upsample2x_bwd": ("din",), "pcm_conv3x3_c4": ("out",),
     "pcm_timestep_embed": ("out",), "pcm_add_bf16": ("out",), "pcm_cast_f32_bf16": ("out",),
     "pcm_grad_sumsq": ("out",), "pcm_adamw_clip": ("p", "g", "m", "v", "state"), "pcm_ema_update": ("targ",),
-    "pcm_lora_refresh": ("opnd",),
+    "pcm_lora_refresh": ("opnd",), "pcm_softmax_rows": ("p",), "pcm_transpose_bf16": ("out",),
+    "pcm_latent_dist": ("mean", "logvar", "std", "sample"), "pcm_vae_dec_in": ("out",),
+    "pcm_image_exit": ("out", "u8"),
 }
 SUMSQ_WS_DOUBLES = 1024
 
@@ -155,6 +163,19 @@ def extents(op, a, table=None):
         opnd = max(max(e["a_fwd"], e["a_t"]) + e["r"] * e["taps"] * e["cin"] for e in rows)
         opnd = max(opnd, max(max(e["sb_fwd"], e["sb_t"]) + e["n"] * e["r"] for e in rows))
         return dict(master=4 * master, table=72 * a["num_entries"], opnd=2 * opnd)
+    if op == "pcm_softmax_rows":
+        return dict(s=4 * ((a["rows"] - 1) * a["lds"] + a["cols"]), p=2 * ((a["rows"] - 1) * a["ldp"] + a["cols"]))
+    if op == "pcm_transpose_bf16":
+        return {"in": 2 * ((a["batch"] - 1) * a["bsi"] + (a["rows"] - 1) * a["ldi"] + a["cols"]),
+                "out": 2 * ((a["batch"] - 1) * a["bso"] + (a["cols"] - 1) * a["ldo"] + a["rows"])}
+    if op == "pcm_latent_dist":
+        n = 16 * a["B"] * a["HW"]
+        return dict(h=2 * n, w=2 * 64, bias=4 * 8, noise=n, mean=n, logvar=n, std=n, sample=n)
+    if op == "pcm_vae_dec_in":
+        return dict(z=16 * a["M"], w=2 * 16, bias=4 * 4, out=16 * a["M"])
+    if op == "pcm_image_exit":
+        n = a["B"] * a["HW"] * a["C"]
+        return dict(x=4 * n, out=4 * n, u8=n)
     raise KeyError(op)
 
 
@@ -381,9 +402,75 @@ def materialise(spec, device, seed=0):
     elif op == "pcm_lora_refresh":
         T.view("master", F32).copy_(_g(g, T.view("master", F32).numel(), 0.05))
         T.view("table", torch.int64, 9 * a["num_entries"]).copy_(torch.tensor(spec["table"], device=device).view(-1))
+    elif op == "pcm_softmax_rows":
+        rows, cols = a["rows"], a["cols"]
+        # attention scores: each row N(0, sigma^2), sigma from 0.5 (flat) to 6 (peaked); the last row shifted
+        # by +90, where exp without the max subtraction overflows fp32
+        sig = 0.5 + 5.5 * torch.rand(rows, 1, generator=g, device=device)
+        s, step = softmax_scores(T), max(1, (1 << 24) // cols)
+        for r0 in range(0, rows, step):
+            r1 = min(rows, r0 + step)
+            s[r0:r1] = _g(g, (r1 - r0) * cols).view(r1 - r0, cols) * sig[r0:r1]
+        s[rows - 1] += 90.0
+    elif op == "pcm_transpose_bf16":
+        v = transpose_views(T)[0]
+        v.copy_(_g(g, v.numel()).view(v.shape).to(BF16))
+    elif op == "pcm_latent_dist":
+        n = a["B"] * a["HW"]
+        # encoder.conv_out pixels, not bf16 values (the kernel rounds its inputs); every 7th pixel 40 times
+        # larger, so moments land past both logvar clamps
+        h = _g(g, 8 * n, 2.0).view(n, 8)
+        h[::7] *= 40.0
+        T.view("h", F32, 8 * n).copy_(h.view(-1))
+        T.view("w", BF16, 64).copy_(_g(g, 64, 0.35).to(BF16))
+        T.view("bias", F32, 8).copy_(_g(g, 8, 0.5))
+        if a["noise"]:
+            T.view("noise", F32, 4 * n).copy_(_g(g, 4 * n))
+    elif op == "pcm_vae_dec_in":
+        M = a["M"]
+        T.view("z", F32, 4 * M).copy_(_g(g, 4 * M))
+        T.view("w", BF16, 16).copy_(_g(g, 16, 0.5).to(BF16))
+        T.view("bias", F32, 4).copy_(_g(g, 4, 0.1))
+    elif op == "pcm_image_exit":
+        n = a["B"] * a["HW"] * a["C"]
+        x = T.view("x", F32, n)
+        x.copy_(_g(g, n, 0.7))                      # |x| > 1 (clamped) in 15 per cent of the values
+        ties = image_exit_ties().to(device)
+        k = min(n, len(ties))
+        x[:k] = ties[:k]                            # v * 255 exactly k + 1/2 (round half to even) ...
+        x[n - k:] = ties[:k].flip(0)                # ... in the first and the last image
     else:
         raise KeyError(op)
     return T
+
+
+def softmax_scores(T):
+    """[rows, cols] fp32 view of a pcm_softmax_rows spec's scores (row stride lds)."""
+    a = T.spec["args"]
+    return T.view("s", F32).as_strided((a["rows"], a["cols"]), (a["lds"], 1))
+
+
+def transpose_views(T):
+    """(input [batch, rows, cols], output [batch, cols, rows]) bf16 views of a pcm_transpose_bf16 spec."""
+    a = T.spec["args"]
+    return (T.view("in", BF16).as_strided((a["batch"], a["rows"], a["cols"]), (a["bsi"], a["ldi"], 1)),
+            T.view("out", BF16).as_strided((a["batch"], a["cols"], a["rows"]), (a["bso"], a["ldo"], 1)))
+
+
+@functools.lru_cache(None)
+def image_exit_ties():
+    """fp32 inputs x whose image value v = x / 2 + 0.5 (fp32) makes v * 255 (fp32) exactly k + 1/2, for
+    every k in [0, 255) that has one: the ties round(v * 255) rounds to even."""
+    out = []
+    for k in range(255):
+        b0 = int(torch.tensor([(k + 0.5) / 255], dtype=F32).view(torch.int32))
+        for b in range(b0 - 8, b0 + 9):                 # the fp32 values within 8 ulps
+            v = torch.tensor([b], dtype=torch.int32).view(F32)
+            x = ((v.double() - 0.5) * 2).float()
+            if float(v * 255) == k + 0.5 and torch.equal(x / 2 + 0.5, v):
+                out.append(float(x))
+                break
+    return torch.tensor(out, dtype=F32)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -758,6 +845,109 @@ def _refresh_ref(spec, Tin, Tout):
         yield Piece("lora_refresh", opnd[e["sb_t"]:e["sb_t"] + n * r], sB.to(BF16).t().reshape(-1))
 
 
+def softmax_depth(cols):
+    """Summation depth of one row sum of csrc/vae.cu softmax_rows_kernel: a float4's four exponentials are
+    added pairwise (2), each thread chains its ceil(cols / 1024) float4s (256 threads of cols / 4 float4s),
+    then the 5-level xor tree of a warp and the 8 warp partials added one after another (7)."""
+    return -(-cols // 1024) + 2 + 5 + 7
+
+
+def _softmax_ref(spec, Tin, Tout):
+    """p = exp(s - max) / sum exp(s - max), bf16, against float64.
+
+    The max is exact.  d = s - max is one fp32 subtraction (error u |d|, which exp turns into a relative
+    u |d|); expf is within 2 ulps (2^-22 relative), plus 2^-149 where it underflows: e_j = exp(d_j) within
+    r_j = (|d_j| + 4) u.  The sum of these positive terms passes through `softmax_depth` roundings, so the
+    kernel's sum is within R = sum_j e_j r_j / sum + (depth + 1) u of the exact one (relative), the IEEE
+    reciprocal and the product add u each: p_j in fp32 is within (r_j + R + 2 u)(1 + 2^-20) p_j + 2^-149
+    of the exact value (the 2^-20 covers the products of first-order terms), then one bf16 rounding."""
+    a = spec["args"]
+    rows, cols = a["rows"], a["cols"]
+    depth = softmax_depth(cols)
+    s = softmax_scores(Tin)
+    p = Tout.view("p", BF16).as_strided((rows, cols), (a["ldp"], 1))
+    step = max(1, (1 << 22) // cols)
+    for r0 in range(0, rows, step):
+        r1 = min(rows, r0 + step)
+        x = s[r0:r1].double()
+        d = x - x.max(1, keepdim=True).values
+        e = d.exp()
+        tot = e.sum(1, keepdim=True)
+        r = (d.abs() + 4) * U
+        R = (e * r).sum(1, keepdim=True) / tot + (depth + 1) * U
+        ref = e / tot
+        yield Piece("softmax", p[r0:r1], ref, bf16_bound(ref, (r + R + 2 * U) * (1 + 2.0 ** -20) * ref + 2.0 ** -149))
+
+
+def _latent_ref(spec, Tin, Tout):
+    """quant_conv and the latent distribution against float64.
+
+    moments = bf16(sum_k bf16(h_k) w_k + bias): the first fma of the chain is exact (a product of two bf16
+    values), the other 7 and the bias add round once each, so the fp32 value is within 8 u S of the exact
+    sum, S = sum |h_k w_k| + |bias|; then one bf16 rounding.  logvar is that, clamped to [-30, 20]: both
+    ends are bf16 values, so a moment past a clamp by more than its bound gives the clamp exactly.
+    std = expf(logvar / 2) on the kernel's own logvar (checked first): the halving is exact, expf within
+    2 ulps.  sample = (mean + std * noise) * scale, three fp32 roundings on the kernel's own mean and std:
+    bit for bit the torch fp32 expression."""
+    a = spec["args"]
+    n = a["B"] * a["HW"]
+    B, HW = a["B"], a["HW"]
+    x = Tin.view("h", F32, 8 * n).view(n, 8).to(BF16).double()
+    w = Tin.view("w", BF16, 64).view(8, 8).double()
+    bias = Tin.view("bias", F32, 8).double()
+    mo = x @ w.t() + bias
+    e = 8 * U * (x.abs() @ w.abs().t() + bias.abs())
+
+    def nchw(t):
+        return t.view(B, HW, 4).permute(0, 2, 1)
+
+    def out(name):
+        return Tout.view(name, F32, 4 * n).view(B, 4, HW)
+    yield Piece("latent_dist mean", out("mean"), nchw(mo[:, :4]), nchw(bf16_bound(mo[:, :4], e[:, :4])))
+    lv = mo[:, 4:]
+    bnd = bf16_bound(lv, e[:, 4:])
+    clamped = lv.clamp(-30.0, 20.0)
+    bnd = torch.where((clamped - lv).abs() > bnd, torch.zeros_like(bnd), bnd)
+    yield Piece("latent_dist logvar", out("logvar"), nchw(clamped), nchw(bnd))
+    sd = (out("logvar").double() / 2).exp()
+    yield Piece("latent_dist std", out("std"), sd, 2.0 ** -22 * sd + 2.0 ** -149)
+    if a["noise"]:
+        noise = Tin.view("noise", F32, 4 * n).view(B, 4, HW)
+        smp = (out("mean") + out("std") * noise) * torch.tensor(f32(a["scale"]), dtype=F32, device=noise.device)
+        yield Piece("latent_dist sample", out("sample"), smp)
+
+
+def _dec_in_ref(spec, Tin, Tout):
+    """post_quant_conv on bf16(z / div) against float64: the input is the IEEE fp32 quotient rounded to
+    bf16 (computed so here); the 4-term fma chain (the first product exact) and the bias add round 4 times,
+    each within u S, S = sum |x_k w_k| + |bias|; then one bf16 rounding.  Channels 4..7 are zero, bit for bit."""
+    a = spec["args"]
+    M = a["M"]
+    z = Tin.view("z", F32, 4 * M).view(M, 4)
+    x = (z / torch.tensor(f32(a["div"]), dtype=F32, device=z.device)).to(BF16).double()
+    w = Tin.view("w", BF16, 16).view(4, 4).double()
+    bias = Tin.view("bias", F32, 4).double()
+    ref = x @ w.t() + bias
+    out = Tout.view("out", BF16, 8 * M).view(M, 8)
+    yield Piece("vae_dec_in", out[:, :4], ref, bf16_bound(ref, 4 * U * (x.abs() @ w.abs().t() + bias.abs())))
+    yield Piece("vae_dec_in zeros", out[:, 4:], torch.zeros(M, 4, dtype=BF16, device=z.device))
+
+
+def _image_exit_ref(spec, Tin, Tout):
+    """v = (x / 2 + 0.5).clamp(0, 1) and round(v * 255) in torch fp32 (x / 2 is exact, each other operation
+    one IEEE rounding; round half to even): bit for bit, fp32 NCHW and uint8 NHWC."""
+    a = spec["args"]
+    B, HW, C = a["B"], a["HW"], a["C"]
+    n = B * HW * C
+    x = Tin.view("x", F32, n)
+    for b in range(B):
+        v = (x[b * HW * C:(b + 1) * HW * C] / 2 + 0.5).clamp(0.0, 1.0)
+        if a["out"]:
+            yield Piece("image_exit f32", Tout.view("out", F32, n).view(B, C, HW)[b], v.view(HW, C).t())
+        if a["u8"]:
+            yield Piece("image_exit u8", Tout.view("u8", torch.uint8, n).view(B, HW * C)[b], (v * 255).round().to(torch.uint8))
+
+
 def reference(spec, Tin, Tout):
     """The Pieces of one launch: every output window of `Tout` against float64 (or exact) results computed
     from the inputs in `Tin` (a snapshot taken before the launch: AdamW and EMA update in place)."""
@@ -808,6 +998,18 @@ def reference(spec, Tin, Tout):
                         + U * ref.abs() + (0 if rate >= 0.5 else U * s.abs()))
     elif op == "pcm_lora_refresh":
         yield from _refresh_ref(spec, Tin, Tout)
+    elif op == "pcm_softmax_rows":
+        yield from _softmax_ref(spec, Tin, Tout)
+    elif op == "pcm_transpose_bf16":
+        x, out = transpose_views(Tin)[0], transpose_views(Tout)[1]
+        for b in range(a["batch"]):
+            yield Piece("transpose", out[b], x[b].t())
+    elif op == "pcm_latent_dist":
+        yield from _latent_ref(spec, Tin, Tout)
+    elif op == "pcm_vae_dec_in":
+        yield from _dec_in_ref(spec, Tin, Tout)
+    elif op == "pcm_image_exit":
+        yield from _image_exit_ref(spec, Tin, Tout)
     else:
         raise KeyError(op)
 
@@ -902,13 +1104,22 @@ def launch(spec, T, **over):
 
 
 def out_windows(spec):
-    """(label, first byte, bytes) of every window the launch may write."""
-    a = spec["args"]
-    ext = extents(spec["op"], a, spec.get("table"))
+    """(label, first byte, bytes) of every window the launch may write.  A strided output (softmax rows
+    ldp apart, transposed rows ldo / bso apart) is one window per row when its rows leave gutters."""
+    op, a = spec["op"], spec["args"]
+    ext = extents(op, a, spec.get("table"))
     wins = []
-    for k in _OUTS[spec["op"]]:
-        if isinstance(a.get(k), list):
-            wins.append((a[k][0], a[k][1], ext[k]))
+    for k in _OUTS[op]:
+        if not isinstance(a.get(k), list):
+            continue
+        lab, off = a[k]
+        if op == "pcm_softmax_rows" and a["ldp"] != a["cols"]:
+            wins += [(lab, off + 2 * r * a["ldp"], 2 * a["cols"]) for r in range(a["rows"])]
+        elif op == "pcm_transpose_bf16" and (a["ldo"] != a["rows"] or a["bso"] != a["cols"] * a["rows"]):
+            wins += [(lab, off + 2 * (b * a["bso"] + c * a["ldo"]), 2 * a["rows"])
+                     for b in range(a["batch"]) for c in range(a["cols"])]
+        else:
+            wins.append((lab, off, ext[k]))
     return wins
 
 
